@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- rendered frames/sec at 64^2 neural x 96 samples -> 512^2 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     (N > 1: python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...)
 
 A "step" is one pass of the hot path over one batch: G.synthesis(ws, c) for 8 latents of the random-init
@@ -18,6 +18,8 @@ roofline : the fused ray-march kernel (dominant kernel of the renderer), timed l
 cpu_baseline : the oracle port (stock torch-CPU ops chained like the reference's free functions) on the host cores,
         bounded sample = 1 frame of the same workload.
 --impl reference : that CPU path as the timed arm (rank 0 only).
+--dump-outputs DIR : after the run, rank 0 writes what the last timed step returned (the [8, 3, 512, 512] frames) as
+        DIR/image.npy (float32); the inputs are seeded, so two builds can be compared output for output.
 """
 
 import argparse
@@ -122,7 +124,7 @@ def measured_peak_gbs():
             return float(json.load(open(p))['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs)'
         except Exception:
             pass
-    return 6650.0, 'fallback (B200_PROFILING.md 6.65 TB/s)'
+    return 3350.0, 'data sheet (H100 SXM HBM3 3.35 TB/s; not measured)'
 
 
 def pick_cpu_threads():
@@ -245,6 +247,7 @@ def main():
     ap.add_argument('--impl', default='ours', choices=['ours', 'reference'])
     ap.add_argument('--cpu-reps', type=int, default=2, help='timed repetitions of the 1-frame CPU baseline')
     ap.add_argument('--no-cpu-baseline', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None, help='write the last timed step\'s output as DIR/image.npy')
     args = ap.parse_args()
 
     if args.impl == 'reference':
@@ -267,7 +270,7 @@ def main():
         ws = G.mapping(z_host.to(device), c_host.to(device))
     c = c_host.to(device)
     kw = dict(render_params=dict(num_steps=NUM_STEPS), noise_mode='const')
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=device)      # 256 MB > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=device)      # 256 MB > the 50 MB L2
 
     def barrier():
         if world > 1:
@@ -297,13 +300,14 @@ def main():
         render.kernel_events = []
         launches0 = _lib.launch_count()
         ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.steps)]
+        torch.manual_seed(1234)                   # the per-step ray jitter seeds come from torch's CPU generator: same every run
         with ClockSampler(device.index or 0) as clocks:
             barrier()
             torch.cuda.profiler.start()           # no-op unless run under `ncu --profile-from-start off`
             for a, b in ev:
                 flush.zero_()
                 a.record()
-                step()
+                last_out = step()
                 b.record()
             barrier()
             torch.cuda.profiler.stop()
@@ -362,13 +366,13 @@ def main():
             'e2e': {'value': e2e_value, 'unit': 'frames/s', 'h2d_bytes_per_step': int((ws_pin.numel() * 4 + c_pin.numel() * 4) // args.steps),
                     'd2h_bytes_per_step': int(BATCH * world * 3 * 512 * 512), 'call': 'ide3d_b200.dist.stream_frames_sharded (pinned host ws/c -> uint8 frames in pinned host memory; D2H of batch i overlaps batch i+1)'},
             'gpu_launches': int(launches),
-            'roofline': {'kernel': 'tc3::raymarch_tc3_kernel (fused gather + tcgen05 decoder MLP, compositing folded into the layer-2 operand)', 'bound': 'hbm', 'achieved': achieved, 'peak': peak, 'unit': 'GB/s',
+            'roofline': {'kernel': 'raymarch_tc_kernel (fused gather + wgmma decoder MLP + compositing)', 'bound': 'hbm', 'achieved': achieved, 'peak': peak, 'unit': 'GB/s',
                          'frac': achieved / peak, 'traffic': traffic, 'traffic_source': traffic_src, 'peak_source': peak_src, 'kernel_ms': kern_ms,
                          'algorithmic_bytes_per_launch': BATCH * FRAME_ALGO_BYTES,
                          'kernel_only_fps': BATCH / (kern_ms * 1e-3), 'renderer_fps_incl_layout_pass': BATCH / (renderer_ms * 1e-3),
                          'reference_gpu_chain_ms': chain_ms, 'vs_reference_gpu_chain': chain_ms / kern_ms,
                          'vs_reference_gpu_chain_note': 'reference renderer op chain (rays, jitter, bmm, 6x grid_sample, decoder matmuls, compositing; every stage in HBM) on this GPU, same planes and decoder, / kernel_ms; north-star target >= 20',
-                         'note': 'HBM is not the limiter of this kernel: 24 texel lines per sample are served by L1/L2 and the kernel is gather-latency bound (profiles/r02k_ncu_raymarch_tc3.txt); frac is reported as the contract asks'},
+                         'note': 'HBM is not the limiter of this kernel: 24 texel lines per sample are served by L1/L2 and the kernel is gather-latency bound; frac is algorithmic bytes over the HBM peak'},
             'clocks': clocks.summary(),
         }
         if not args.no_cpu_baseline and world == 1:
@@ -383,6 +387,9 @@ def main():
                               'uint8_mean_levels': float(lv.float().mean()), 'tolerance': 'tests/test_gpu_fullsize.py: image 1e-2 x max|ref| under TF32 (1e-4 with fp32 convolutions)'}
             line['cpu_baseline'] = {'value': fps, 'unit': 'frames/s', 'cores': torch.get_num_threads(), 'kind': 'port',
                                     'sample': f'1 frame of the batch (full synthesis, {sec:.1f} s each, {args.cpu_reps} reps + 1 warm-up), oracle port on torch-CPU ops'}
+        if args.dump_outputs:
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            np.save(os.path.join(args.dump_outputs, 'image.npy'), last_out.float().cpu().numpy())
         print(json.dumps(line))
     if world > 1:
         tdist.barrier()

@@ -1,7 +1,7 @@
-"""ide3d_b200 -- B200-native implementation of IDE-3D's volumetric-rendering hot path.
+"""ide3d_b200 -- H100-native implementation of IDE-3D's volumetric-rendering hot path.
 
 Layout (mirrors the reference's module names so its tools can import this package instead):
-    csrc/                     hand-written sm_100a CUDA + the C-ABI (include/ide3d_b200.h)
+    csrc/                     hand-written sm_90a CUDA + the C-ABI (include/ide3d_b200.h)
     _lib.py, _plugins.py      ctypes binding, plugin-level functions (the pybind11 surface of the reference)
     torch_utils/ops/*         bias_act, upfirdn2d, filtered_lrelu, conv2d_gradfix, conv2d_resample, fma, grid_sample_gradfix
     torch_utils/custom_ops.py get_plugin()

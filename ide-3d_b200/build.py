@@ -1,9 +1,9 @@
-"""Build libide3d_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libide3d_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
     python ide-3d_b200/build.py [--force] [--verbose]
 
 No torch involvement: plain `nvcc -c` per translation unit (in parallel) and one `nvcc -shared` link.
-The result lands in ide-3d_b200/lib/libide3d_b200.so; it is git-ignored but travels with gpurun snapshots.
+The result lands in ide-3d_b200/lib/libide3d_b200.so (git-ignored build product).
 """
 
 import hashlib
@@ -18,9 +18,9 @@ CSRC = os.path.join(HERE, 'csrc')
 OBJ = os.path.join(HERE, '_build_tuning' if os.environ.get('IDE3D_BUILD_TUNING', '0') == '1' else '_build')
 LIBDIR = os.path.join(HERE, 'lib')
 LIB = os.path.join(LIBDIR, 'libide3d_b200_tuning.so' if os.environ.get('IDE3D_BUILD_TUNING', '0') == '1' else 'libide3d_b200.so')
-TUNING = os.environ.get('IDE3D_BUILD_TUNING', '0') == '1'      # experiment switches + the round-1 ray-march kernel (A/B scripts only)
-UNITS = ['capi', 'raymarch', 'raymarch_bwd', 'raymarch_tc', 'raymarch_tc3'] + (['raymarch_tc_v1'] if TUNING else []) + [ 'voxel', 'voxel_tc', 'stages', 'style_plan', 'mcubes', 'bias_act', 'upfirdn2d', 'filtered_lrelu', 'filtered_lrelu_fused']
-NVCC_FLAGS = ['-O3', '-std=c++17', '--expt-relaxed-constexpr', '-gencode', 'arch=compute_100a,code=sm_100a',
+TUNING = os.environ.get('IDE3D_BUILD_TUNING', '0') == '1'      # experiment switches (A/B scripts only)
+UNITS = ['capi', 'raymarch', 'raymarch_bwd', 'raymarch_tc', 'voxel', 'voxel_tc', 'stages', 'style_plan', 'mcubes', 'bias_act', 'upfirdn2d', 'filtered_lrelu', 'filtered_lrelu_fused']
+NVCC_FLAGS = ['-O3', '-std=c++17', '--expt-relaxed-constexpr', '-gencode', 'arch=compute_90a,code=sm_90a',
               '-lineinfo', '-Xcompiler', '-fPIC', '-Xptxas', '-v'] + (['-DIDE3D_TUNING'] if TUNING else [])
 
 
@@ -72,7 +72,7 @@ def build(force=False, verbose=False):
     units = _sources()
     with ThreadPoolExecutor(max_workers=min(8, len(units))) as ex:
         objs = list(ex.map(lambda u: _compile(nvcc, u, verbose), units))
-    cmd = [nvcc, '-shared', '-gencode', 'arch=compute_100a,code=sm_100a', '-o', LIB] + objs + ['-lcudart']
+    cmd = [nvcc, '-shared', '-gencode', 'arch=compute_90a,code=sm_90a', '-o', LIB] + objs + ['-lcudart']
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError('link failed:\n' + r.stdout)

@@ -3,7 +3,7 @@
     import ide3d_b200.compat as compat; compat.install()
 
 After install(), `from training.volumetric_rendering import sample_camera_positions`, `from training.triplane
-import TriPlaneGenerator`, `from torch_utils.ops import upfirdn2d`, `import dnnlib` ... resolve to the sm_100a
+import TriPlaneGenerator`, `from torch_utils.ops import upfirdn2d`, `import dnnlib` ... resolve to the sm_90a
 implementations, so gen_images.py / gen_videos.py / extract_shapes.py / viz/renderer.py run unchanged against a
 generator built by `random_init_generator()` (the reference checkpoints embed their own class source and are not
 available offline; see INTEGRATION.md).

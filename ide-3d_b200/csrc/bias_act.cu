@@ -1,4 +1,4 @@
-// bias_act for sm_100a: y = clamp(gain * act(x + b)) plus the 1st/2nd-order gradient forms.
+// bias_act for sm_90a: y = clamp(gain * act(x + b)) plus the 1st/2nd-order gradient forms.
 // Replaces bias_act_kernel<T,A> (torch_utils/ops/bias_act.cu:23-147) behind the same parameter set
 // (bias_act.h:12-31).  Pure HBM stream: 2 * size_x * sizeof(T) algorithmic bytes (+ aux tensors for
 // the gradient forms).  128-bit loads/stores, 4 vectors in flight per thread, 64-bit indexing, grid
@@ -384,7 +384,7 @@ __global__ void __launch_bounds__(256) modconv_epilogue_planar_kernel(const EpiA
 // channels_last: one 16-byte vector = N consecutive channels of one pixel; scale / bias are vectors, the noise a scalar.
 // Work items are (sample, chunk of 256*UNROLL vectors): the sample index is block-uniform and the position inside the
 // sample fits 32 bits, so the per-vector index math is one shift/mask (power-of-two channel counts) or one 32-bit division
-// -- the first version spent 3/4 of its issue slots on 64-bit div/mod (profiles/r01_ncu_modconv_epilogue.txt).
+// -- the first version spent 3/4 of its issue slots on 64-bit div/mod.
 template <typename T, int A, int UNROLL>
 __global__ void __launch_bounds__(256) modconv_epilogue_cl_kernel(const EpiArgs p, unsigned chunks_per_sample, long long items, int cv_shift) {
     using S = typename Acc<T>::type;

@@ -1,4 +1,4 @@
-// Shared helpers for libide3d_b200.so (sm_100a).  No torch, no global device state.
+// Shared helpers for libide3d_b200.so (sm_90a).  No torch, no global device state.
 #pragma once
 
 #include <cuda_fp16.h>
@@ -56,11 +56,11 @@ inline const char* tuning_env(const char* name) {
 inline int sm_count() {
     static thread_local int cached_dev = -1, cached = 0;
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
     if (dev != cached_dev) {
         cudaDeviceGetAttribute(&cached, cudaDevAttrMultiProcessorCount, dev);
         cached_dev = dev;
-        if (cached <= 0) cached = 148;
+        if (cached <= 0) cached = 132;
     }
     return cached;
 }

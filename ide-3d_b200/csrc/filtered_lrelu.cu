@@ -1,4 +1,4 @@
-// filtered_lrelu for sm_100a.
+// filtered_lrelu for sm_90a.
 //   ide3d_filtered_lrelu_act : in-place gain * lrelu * clamp with 2-bit sign write / read -- the activation
 //                              stage of the generic composition (filtered_lrelu.cu:1105-1211,
 //                              filtered_lrelu.cpp:213-290).

@@ -1,4 +1,4 @@
-// Fused filtered_lrelu for sm_100a: bias -> up-FIR -> gain * leaky ReLU * clamp (+ 2-bit signs) -> down-FIR in ONE kernel for
+// Fused filtered_lrelu for sm_90a: bias -> up-FIR -> gain * leaky ReLU * clamp (+ 2-bit signs) -> down-FIR in ONE kernel for
 // separable filters (filtered_lrelu.cu:139-1099 of the reference; its CASE table :1248-1278).  Round-2 design.
 //
 // A CTA owns a TOW x TOH output tile of CB channels; the up^2-sized intermediate never leaves the SM.  The four separable

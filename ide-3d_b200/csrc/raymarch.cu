@@ -195,9 +195,6 @@ static int launch_raymarch(const RayArgs& a, cudaStream_t st) {
 }
 
 int launch_raymarch_tc(const ide3d_raymarch_params* p, bool channels_last, cudaStream_t st);   // raymarch_tc.cu
-#ifdef IDE3D_TUNING
-namespace v1 { int launch_raymarch_tc_v1(const ide3d_raymarch_params* p, bool channels_last, cudaStream_t st); }   // raymarch_tc_v1.cu (round-1 kernel, A/B only)
-#endif
 
 }  // namespace ide3d
 
@@ -232,13 +229,7 @@ extern "C" int ide3d_raymarch_fwd(const ide3d_raymarch_params* p, ide3d_stream_t
     IDE3D_REQUIRE(p->precision >= IDE3D_PRECISION_AUTO && p->precision <= IDE3D_PRECISION_TC, "raymarch: bad precision");
     const bool planes_cl = is_channels_last(p->tex) && is_channels_last(p->seg);
     if (p->precision != IDE3D_PRECISION_FP32) {
-#ifdef IDE3D_TUNING
-        const char* v1 = tuning_env("IDE3D_TC_V1");              // the round-1 kernel, linked into tuning builds only (A/B baseline)
-        const int rc_tc = (v1 && v1[0] == '1') ? v1::launch_raymarch_tc_v1(p, planes_cl, (cudaStream_t)stream)
-                                               : launch_raymarch_tc(p, planes_cl, (cudaStream_t)stream);
-#else
         const int rc_tc = launch_raymarch_tc(p, planes_cl, (cudaStream_t)stream);
-#endif
         if (rc_tc != IDE3D_UNSUPPORTED || p->precision == IDE3D_PRECISION_TC) return rc_tc;
     }
     const int kind = classify_decoder(p->dec);

@@ -149,7 +149,7 @@ __device__ __forceinline__ void gather_chunk_to(const PlaneView& tex, const Plan
     }
 }
 
-// Per-axis form of the same gather (tcgen05 producers): the three planes share their axes -- x is the column of planes 0 and
+// Per-axis form of the same gather (tensor-core kernels): the three planes share their axes -- x is the column of planes 0 and
 // 2, y the row of plane 0 and the column of plane 1, z the row of planes 1 and 2 -- so the floor / fraction / validity /
 // clamp work is done once per axis role (4 roles) instead of once per tap (12 taps), and a tap's offset and weight are one
 // add and one multiply.  Same arithmetic as the per-tap form above: w = (x-weight or 0) * (y-weight or 0), identical products.

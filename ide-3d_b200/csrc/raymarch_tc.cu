@@ -1,54 +1,76 @@
-// Fused volume renderer, tensor-core decoder (round-2 design): rays -> jitter -> cam2world -> 2x tri-plane gather -> decoder MLP
-// -> alpha compositing in ONE kernel, no per-sample intermediate in HBM (training/volumetric_rendering.py:34-136,
-// dnnlib/util.py:580-617 and the generator's decoder in one pass).
+// Fused volume renderer, tensor-core decoder: rays -> jitter -> cam2world -> 2x tri-plane gather -> decoder MLP -> alpha compositing
+// in ONE kernel, no per-sample intermediate in HBM (training/volumetric_rendering.py:34-136, dnnlib/util.py:580-617 and the
+// generator's decoder in one pass).
 //
-//   unit   = 4x4 neighbouring rays, marched front to back; tile = 8 consecutive depth samples of the 16 rays = 128 rows (M = 128)
-//            row r: warp quarter r/32 = pixel row of the unit, lane = (pixel column)*8 + depth index   -> the 8 samples of a ray
-//            sit in 8 adjacent lanes (compositing = 8-lane segmented product), rays that share a plane row / column share texels
-//   A      = gathered features [128 x 64] (texture 0..31 | shape 32..63), bf16 hi + lo, K-major, 128B-swizzled smem rows
-//   layer 1: D1[128 x 64] per hidden block = A . W1_blk^T, fp32 accumulators in TMEM
-//   epilog : tcgen05.ld D1 -> + b1 -> softplus -> bf16 hi / lo -> tcgen05.st back INTO THE SAME TMEM COLUMNS (16 fp32 columns
-//            become 8 packed hi + 8 packed lo columns: one K = 16 step)
-//   layer 2: D2[128 x n] (+)= A2 . W2_blk^T with the A operand read FROM TMEM (tcgen05.mma [d], [a_tmem], b_desc): no shared-memory
-//            round trip, no proxy fence, no block-wide barrier between the two layers
-//   final  : tcgen05.ld D2 -> + b2 -> sigma -> alpha -> 8-lane product scan (+ carried transmittance) -> weighted accumulation in
-//            registers; one 8-lane reduction per ray at the end of the march
+//   unit   = 4x2 neighbouring rays, marched front to back by one warpgroup; tile = 8 consecutive depth samples of the 8 rays = 64 rows
+//            warp w of the warpgroup owns rows 16w..16w+15: rays (2(w%2), w/2) and (2(w%2)+1, w/2), row = 8 * ray + depth index.
+//            That is the row ownership of the wgmma accumulator (lane l holds rows l/4 and l/4 + 8), so a lane holds the same depth
+//            sample of both of its warp's rays and the 8 samples of a ray sit in the 8 lanes l%4 == const (compositing = 8-lane scan)
+//   A      = gathered features [64 x 64] (texture 0..31 | shape 32..63), bf16 hi + lo, K-major, 128B-swizzled smem rows; every warp
+//            gathers its own 16 rows (8 lanes per texel x LDG.128), one named barrier per tile hands the tile to the warpgroup MMA
+//   layer 1: D1[64 x 64] per hidden block = A . W1_blk^T, wgmma with both operands in shared memory, fp32 accumulators in registers
+//   epilog : + b1 -> softplus -> bf16 hi / lo, repacked in registers as the A fragments of layer 2 (accumulator and A fragment share
+//            their row / column ownership): no shared-memory round trip between the layers
+//   layer 2: D2[64 x n] += A2 . W2_blk^T, wgmma with the A operand in registers, over the output columns the block feeds
+//   final  : + b2 -> sigma -> alpha -> 8-lane product scan (+ carried transmittance) -> weighted accumulation in registers; one
+//            8-lane reduction per ray at the end of the march
 // Every product is bf16 hi*hi + hi*lo + lo*hi with fp32 accumulation ("bf16x3": 16 mantissa bits per operand).
 //
-// Warp-specialised persistent CTA, 640 threads, one CTA per SM:
-//   warps 0-3 / 4-7    two consumer GROUPS; a group owns 256 TMEM columns (D1 3x64 + D2 64) and marches its own units, so the MMA /
-//                      commit latency of one group's tile is covered by the softplus / compositing work of the other group;
-//                      lane 0 of a group's first warp issues its MMAs
-//   warps 8-19         producers, three teams of four warps; a team fills one 32 KB A stage (a tile) at a time: sample positions,
-//                      per-axis bilinear footprints (once per sample, by the lane that owns it), 8 lanes per texel x LDG.128,
-//                      blend, bf16 split, swizzled st.shared; mbarrier full / empty ring, "empty" = tcgen05.commit of layer 1
-// Shared memory: compacted weight tiles (52 KB for the three-head decoder) + kStages x 32 KB, so that 64+ KB stay L1 for the gather.
+// CTA = two warpgroups that share the weight tiles in shared memory (compacted: 52 KB for the three-head decoder) and march
+// independent units, so the gather latency of one is covered by the MMA / softplus / compositing work of the other and of the
+// other resident CTAs.
 #include "raymarch_tc_shared.cuh"
 
 namespace ide3d {
 
-template <int TEAMS>
-__global__ void __launch_bounds__(TcCfg<TEAMS>::kThreads, 1) raymarch_tc_kernel(const TcArgs a) {
-    constexpr int kStages = TEAMS, kTeams = TEAMS, kTcThreads = TcCfg<TEAMS>::kThreads;
+// layer 2 of one hidden block into D2 columns [N0, N0 + N)
+template <int N0, int N>
+__device__ __forceinline__ void layer2(float (&d2)[32], const uint32_t (&ah)[4][4], const uint32_t (&al)[4][4], uint64_t wh, uint64_t wl) {
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {
+        tc::Wgmma<N>::rs(d2 + N0 / 2, ah[ks], wh + ks * 2);
+        tc::Wgmma<N>::rs(d2 + N0 / 2, ah[ks], wl + ks * 2);
+        tc::Wgmma<N>::rs(d2 + N0 / 2, al[ks], wh + ks * 2);
+    }
+}
+
+__device__ __forceinline__ void layer2_cols(int n0, int n, float (&d2)[32], const uint32_t (&ah)[4][4], const uint32_t (&al)[4][4],
+                                            uint64_t wh, uint64_t wl) {
+    switch ((n0 >> 4) * 4 + (n >> 4) - 1) {
+        case 0: layer2<0, 16>(d2, ah, al, wh, wl); break;
+        case 1: layer2<0, 32>(d2, ah, al, wh, wl); break;
+        case 2: layer2<0, 48>(d2, ah, al, wh, wl); break;
+        case 3: layer2<0, 64>(d2, ah, al, wh, wl); break;
+        case 4: layer2<16, 16>(d2, ah, al, wh, wl); break;
+        case 5: layer2<16, 32>(d2, ah, al, wh, wl); break;
+        case 6: layer2<16, 48>(d2, ah, al, wh, wl); break;
+        case 8: layer2<32, 16>(d2, ah, al, wh, wl); break;
+        case 9: layer2<32, 32>(d2, ah, al, wh, wl); break;
+        case 12: layer2<48, 16>(d2, ah, al, wh, wl); break;
+        default: break;                                                  // excluded by build_program (columns within 0..63)
+    }
+}
+
+__device__ __forceinline__ void fence_frag(uint32_t (&f)[4][4]) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) asm volatile("" : "+r"(f[i][j])::"memory");
+}
+
+__global__ void __launch_bounds__(kTcThreads) raymarch_tc_kernel(const TcArgs a) {
     extern __shared__ unsigned char smem_raw[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     const TcProgram& P = a.prog;
     unsigned char* w_hi = smem;
     unsigned char* w_lo = smem + P.wpart;
-    unsigned char* stage_base = smem + 2 * P.wpart;
-    unsigned char* misc = stage_base + kStages * kStageBytes;
-    float* b1s = reinterpret_cast<float*>(misc);                         // [3 x 64] hidden biases (x log2e)
-    float* b2s = b1s + kTcMaxBlocks * 64;                                 // [64] output biases
-    uint64_t* bar_full = reinterpret_cast<uint64_t*>(b2s + 64);         // [kStages] producer team -> consumers
-    uint64_t* bar_empty = bar_full + kMaxTeams;                      // [kStages] layer-1 commit -> producers
-    uint64_t* bar_d1 = bar_empty + kMaxTeams;                        // [kGroups] layer 1 done
-    uint64_t* bar_a2 = bar_d1 + kGroups;                                // [kGroups][kTcMaxBlocks] A2 of a hidden block is in TMEM (4 warp arrivals)
-    uint64_t* bar_d2 = bar_a2 + kGroups * kTcMaxBlocks;                 // [kGroups] layer 2 done
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_d2 + kGroups);
+    unsigned char* tile_base = smem + 2 * P.wpart;
+    float* b1s = reinterpret_cast<float*>(tile_base + kWarpgroups * kStageBytes);   // [3 x 64] hidden biases (x log2e)
+    float* b2s = b1s + kTcMaxBlocks * 64;                                            // [64] output biases
 
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tid = threadIdx.x, lane = tid & 31;
 
-    // ---------------- one-time setup: weights -> bf16 hi/lo swizzled tiles (compacted), biases, barriers, TMEM
+    // ---------------- one-time setup: weights -> bf16 hi/lo swizzled tiles (compacted), biases
     for (int i = tid; i < (2 * P.wpart) / 16; i += kTcThreads) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
     __syncthreads();
     for (int i = tid; i < P.nblocks * 64 * 64; i += kTcThreads) {
@@ -77,235 +99,189 @@ __global__ void __launch_bounds__(TcCfg<TEAMS>::kThreads, 1) raymarch_tc_kernel(
         }
         b2s[tid] = v;
     }
-    if (tid == 0) {
-        for (int i = 0; i < kStages; ++i) { tc::mbar_init(&bar_full[i], 4); tc::mbar_init(&bar_empty[i], 1); }
-        for (int g = 0; g < kGroups; ++g) { tc::mbar_init(&bar_d1[g], 1); tc::mbar_init(&bar_d2[g], 1); }
-        for (int i = 0; i < kGroups * kTcMaxBlocks; ++i) tc::mbar_init(&bar_a2[i], 4);
-        tc::fence_mbar_init();
-    }
-    if (warp == 0) tc::tmem_alloc(tmem_slot, kGroups * kGroupCols);
     tc::fence_async_smem();
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     const int S = a.steps;
-    const Schedule sch = make_schedule(a);
-    const int unit_stride = kGroups * gridDim.x;
+    const int wg = tid >> 7, w = (tid >> 5) & 3;
+    const int g = lane >> 2, c = lane & 3;                               // accumulator rows g / g + 8, columns 8j + 2c + {0, 1}
+    const int q4 = lane & 7, grp = lane >> 3, l16 = lane & 15;           // gather: channel quad, sample of the instruction, own row
+    const int shb = (int)(a.tex.sh * 4), swb = (int)(a.tex.sw * 4);     // strides in bytes (32-bit: checked by the launcher)
+    const int W = a.tex.w, H = a.tex.h;
+    unsigned char* a_hi = tile_base + wg * kStageBytes;
+    unsigned char* a_lo = a_hi + kTileBytes;
+    const uint64_t ah0 = tc::make_sdesc_sw128(tc::smem_u32(a_hi)), al0 = tc::make_sdesc_sw128(tc::smem_u32(a_lo));
+    const uint64_t wh0 = tc::make_sdesc_sw128(tc::smem_u32(w_hi)), wl0 = tc::make_sdesc_sw128(tc::smem_u32(w_lo));
+    const int unit_stride = kWarpgroups * gridDim.x;
 
-    if (warp >= kConsumerWarps) {
-        // =========================================================================== producers
-        if constexpr (TcCfg<TEAMS>::kProducerRegs < TcCfg<TEAMS>::kBaseRegs) tc::setmaxnreg_dec<TcCfg<TEAMS>::kProducerRegs>();
-        else if constexpr (TcCfg<TEAMS>::kProducerRegs > TcCfg<TEAMS>::kBaseRegs) tc::setmaxnreg_inc<TcCfg<TEAMS>::kProducerRegs>();
-        producer_loop<TEAMS>(a, sch, stage_base, bar_full, bar_empty, warp - kConsumerWarps, lane);
-    } else {
-        // =========================================================================== consumers
-        if constexpr (TcCfg<TEAMS>::kConsumerRegs < TcCfg<TEAMS>::kBaseRegs) tc::setmaxnreg_dec<TcCfg<TEAMS>::kConsumerRegs>();
-        else if constexpr (TcCfg<TEAMS>::kConsumerRegs > TcCfg<TEAMS>::kBaseRegs) tc::setmaxnreg_inc<TcCfg<TEAMS>::kConsumerRegs>();
-        const int g = warp >> 2, qw = warp & 3;
-        const uint32_t d1_col = tmem_base + g * kGroupCols, d2_col = d1_col + kD2Col;
-        const uint32_t lane_sel = (uint32_t)(qw * 32) << 16;
-        const uint32_t w_hi_u = tc::smem_u32(w_hi), w_lo_u = tc::smem_u32(w_lo);
-        const uint32_t stage_u = tc::smem_u32(stage_base);
-        const bool issuer = (qw == 0 && lane == 0);
-        const int seg0 = lane & ~7, d = lane & 7;
-        const int my_tiles = g ? sch.tiles1 : sch.tiles0, my_units = g ? sch.cnt1 : sch.cnt0;
-        uint32_t par_d1 = 0, par_d2 = 0, par_a2 = 0;
+    for (int unit = blockIdx.x * kWarpgroups + wg; unit < a.num_units; unit += unit_stride) {
+        const RaySetup rA = ray_setup(a, unit, (w & 1) * 2, w >> 1);
+        const RaySetup rB = ray_setup(a, unit, (w & 1) * 2 + 1, w >> 1);
+        const RaySetup rG = ray_setup(a, unit, (w & 1) * 2 + (l16 >> 3), w >> 1);      // the ray of this lane's gather row
+        const char* tb = reinterpret_cast<const char*>(a.tex.base + (long long)rG.n * a.tex.sn);
+        const char* sb = reinterpret_cast<const char*>(a.seg.base + (long long)rG.n * a.seg.sn);
+        float acc[2][16];
+#pragma unroll
+        for (int i = 0; i < 16; ++i) acc[0][i] = acc[1][i] = 0.f;
+        float acc_w[2] = {0.f, 0.f}, acc_d[2] = {0.f, 0.f}, T_in[2] = {1.f, 1.f};
 
-        // layer 1 of every hidden block of one tile (D1 has a 64-column slot per block); the A stage is free when these MMAs are done
-        auto issue_l1 = [&](int seq) {
-            const int stage = seq % kStages;
-            const uint32_t a_hi_u = stage_u + stage * kStageBytes, a_lo_u = a_hi_u + kTileBytes;
-            const uint32_t idesc = tc::make_idesc_bf16(128, 64);
+        for (int step = 0; step < a.tiles_per_unit; ++step) {
+            // ---- gather: this lane's sample position, per-axis bilinear footprints (dnnlib/util.py:589-596: plane 0 = (x,y),
+            //      plane 1 = (y,z), plane 2 = (x,z)), computed once per sample; the 8 lanes that fetch a texel receive them by shuffle
+            {
+                const int s = step * kTileDepth + (l16 & 7);
+                float cx = 4.f, cy = 4.f, cz = 4.f;                            // far outside the planes: every tap gets weight 0
+                if (rG.ok && s < S) {
+                    const float* M = a.cam2world + rG.n * 16;
+                    float z0, off0, z1;
+                    sample_depths(a, rG, s, z0, off0, z1);
+                    const float pcx = rG.dx * z0 + off0 * rG.dx, pcy = rG.dy * z0 + off0 * rG.dy, pcz = rG.dz * z0 + off0 * rG.dz;
+                    cx = (M[0] * pcx + M[1] * pcy + M[2] * pcz + M[3]) * a.box_scale;
+                    cy = (M[4] * pcx + M[5] * pcy + M[6] * pcz + M[7]) * a.box_scale;
+                    cz = (M[8] * pcx + M[9] * pcy + M[10] * pcz + M[11]) * a.box_scale;
+                }
+                const AxisFoot fx = axis_foot(cx, W), fyr = axis_foot(cy, H), fyc = axis_foot(cy, W), fz = axis_foot(cz, H);
+                const AxisTaps mX = axis_taps(fx.i0, fx.f, W, swb), mYr = axis_taps(fyr.i0, fyr.f, H, shb);
+                const AxisTaps mYc = axis_taps(fyc.i0, fyc.f, W, swb), mZ = axis_taps(fz.i0, fz.f, H, shb);
+#pragma unroll 1
+                for (int it = 0; it < 4; ++it) {
+                    const int src = it * 4 + grp;                              // 4 depth-consecutive samples of one ray per instruction
+                    AxisTaps X = shfl_taps(mX, src), Yc = shfl_taps(mYc, src);
+                    const AxisTaps Yr = shfl_taps(mYr, src), Z = shfl_taps(mZ, src);
+                    X.lo += q4 * 16; X.hi += q4 * 16; Yc.lo += q4 * 16; Yc.hi += q4 * 16;      // this lane's channel quad
+                    const int row = w * 16 + src;
+                    const uint32_t o_tex = tc::sw128_offset(row, q4 >> 1) + (q4 & 1) * 8;
+                    const uint32_t o_seg = tc::sw128_offset(row, 4 + (q4 >> 1)) + (q4 & 1) * 8;
+                    float f[4];
+                    uint2 hi, lo;
+                    gather12(tb, X, Yr, Yc, Z, f);
+                    tc::split4_bf16(f, hi, lo);
+                    // the tile is overwritten only when every warp of the warpgroup is past the MMAs of the previous tile; the first
+                    // loads of this tile are already in flight
+                    if (it == 0) tc::bar_sync(1 + wg, 128);
+                    *reinterpret_cast<uint2*>(a_hi + o_tex) = hi;
+                    *reinterpret_cast<uint2*>(a_lo + o_tex) = lo;
+                    gather12(sb, X, Yr, Yc, Z, f);
+                    tc::split4_bf16(f, hi, lo);
+                    *reinterpret_cast<uint2*>(a_hi + o_seg) = hi;
+                    *reinterpret_cast<uint2*>(a_lo + o_seg) = lo;
+                }
+                tc::fence_async_smem();                                        // my generic-proxy stores -> async proxy (wgmma)
+                tc::bar_sync(1 + wg, 128);
+            }
+
+            // ---- decoder: per hidden block, layer 1 (smem x smem) -> softplus -> layer 2 (registers x smem) into D2
+            float d2[32];
+#pragma unroll
+            for (int i = 0; i < 32; ++i) d2[i] = 0.f;
             for (int b = 0; b < P.nblocks; ++b) {
                 const TcBlock& B = P.blk[b];
-                const int ks0 = B.k0 >> 4, ksn = B.kcount >> 4;
-                for (int ks = 0; ks < ksn; ++ks) {
-                    const uint32_t off = (uint32_t)(ks0 + ks) * 32;                 // 16 bf16 = 32 bytes along K, same column in A and W1
-                    const uint64_t ah = tc::make_sdesc_sw128(a_hi_u + off), al = tc::make_sdesc_sw128(a_lo_u + off);
-                    const uint64_t wh = tc::make_sdesc_sw128(w_hi_u + B.w1_off + off), wl = tc::make_sdesc_sw128(w_lo_u + B.w1_off + off);
-                    tc::umma_bf16(d1_col + b * 64, ah, wh, idesc, ks > 0);
-                    tc::umma_bf16(d1_col + b * 64, ah, wl, idesc, 1);
-                    tc::umma_bf16(d1_col + b * 64, al, wh, idesc, 1);
-                }
-            }
-            tc::umma_commit(&bar_d1[g]);
-            tc::umma_commit(&bar_empty[stage]);
-        };
-        // layer 2 of one hidden block: A2 (bf16 hi / lo, packed) is read from TMEM columns [64b + 16ks, +8) / [64b + 16ks + 8, +8)
-        auto issue_l2 = [&](int b) {
-            const TcBlock& B = P.blk[b];
-            for (int rr = 0; rr < B.nruns; ++rr) {
-                const TcRun& R = B.runs[rr];
-                const uint32_t idesc = tc::make_idesc_bf16(128, R.n);
-                const uint32_t rowoff = (uint32_t)(R.n0 - B.w2_row0) * 128;          // multiples of 16 rows: 1024-byte atom aligned
-                for (int ks = 0; ks < 4; ++ks) {
-                    const uint32_t off = B.w2_off + rowoff + (uint32_t)ks * 32;
-                    const uint32_t ahi = d1_col + b * 64 + ks * 16, alo = ahi + 8;
-                    const uint64_t wh = tc::make_sdesc_sw128(w_hi_u + off), wl = tc::make_sdesc_sw128(w_lo_u + off);
-                    tc::umma_bf16_ts(d2_col + R.n0, ahi, wh, idesc, (R.accum || ks > 0));
-                    tc::umma_bf16_ts(d2_col + R.n0, ahi, wl, idesc, 1);
-                    tc::umma_bf16_ts(d2_col + R.n0, alo, wh, idesc, 1);
-                }
-            }
-        };
-
-        bool l1_issued = false;                              // layer 1 of the NEXT tile already in flight (issuer only)
-        int t = 0;
-        for (int ui = 0; ui < my_units; ++ui) {
-            const int unit = blockIdx.x * kGroups + g + ui * unit_stride;
-            const RaySetup r = ray_setup(a, unit, lane >> 3, qw);
-            float acc[kOut - 1];
-#pragma unroll
-            for (int c = 0; c < kOut - 1; ++c) acc[c] = 0.f;
-            float acc_w = 0.f, acc_d = 0.f, T_in = 1.f;
-
-            for (int step = 0; step < a.tiles_per_unit; ++step, ++t) {
-                if (issuer && !l1_issued) {
-                    const int seq = seq_of(sch, g, t);
-                    tc::mbar_wait(&bar_full[seq % kStages], (seq / kStages) & 1);
-                    tc::tc_fence_after();
-                    issue_l1(seq);
-                }
-                l1_issued = false;
-                __syncwarp();
-                tc::mbar_wait(&bar_d1[g], par_d1);
-                par_d1 ^= 1;
-                tc::tc_fence_after();
-
-                // ---- hidden blocks: softplus epilogue in place, 16 columns at a time, then layer 2 of the block
-                for (int b = 0; b < P.nblocks; ++b) {
-                    const float* bb = b1s + b * 64;
-#pragma unroll
-                    for (int c16 = 0; c16 < 4; ++c16) {
-                        const uint32_t col = d1_col + b * 64 + c16 * 16 + lane_sel;
-                        float v[16];
-                        tc::tmem_ld16(col, v);
-                        uint32_t ph[8], pl[8];
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const float h0 = softplus2(v[2 * j] + bb[c16 * 16 + 2 * j]);
-                            const float h1 = softplus2(v[2 * j + 1] + bb[c16 * 16 + 2 * j + 1]);
-                            const __nv_bfloat162 hh = __floats2bfloat162_rn(h0, h1);
-                            const float2 back = __bfloat1622float2(hh);
-                            const __nv_bfloat162 ll = __floats2bfloat162_rn(h0 - back.x, h1 - back.y);
-                            ph[j] = *reinterpret_cast<const uint32_t*>(&hh);
-                            pl[j] = *reinterpret_cast<const uint32_t*>(&ll);
-                        }
-                        tc::tmem_st8(col, ph);
-                        tc::tmem_st8(col + 8, pl);
-                    }
-                    tc::tmem_wait_st();
-                    tc::tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) tc::mbar_arrive(&bar_a2[g * kTcMaxBlocks + b]);
-                    if (qw == 0) {
-                        if (lane == 0) {
-                            tc::mbar_wait(&bar_a2[g * kTcMaxBlocks + b], par_a2);
-                            tc::tc_fence_after();
-                            issue_l2(b);
-                            if (b == P.nblocks - 1) {
-                                tc::umma_commit(&bar_d2[g]);
-                                // layer 1 of this group's next tile right behind (MMAs execute in issue order: it overwrites D1 only
-                                // after layer 2 above has read A2 from it) -- if its stage is already full; else after the epilogue
-                                if (t + 1 < my_tiles) {
-                                    const int seq = seq_of(sch, g, t + 1);
-                                    if (tc::mbar_try_wait(&bar_full[seq % kStages], (seq / kStages) & 1)) {
-                                        tc::tc_fence_after();
-                                        issue_l1(seq);
-                                        l1_issued = true;
-                                    }
-                                }
-                            }
-                        }
-                        __syncwarp();
-                    }
-                }
-                par_a2 ^= 1;                             // every a2 barrier completes once per tile
-
-                tc::mbar_wait(&bar_d2[g], par_d2);
-                par_d2 ^= 1;
-                tc::tc_fence_after();
-
-                // ---- sigma + semantic logits (D2 columns 32..55), compositing weight of this sample
-                const int s = step * kTileDepth + d;
-                const bool live = r.ok && (s < S);
-                float z0 = 0.f, off0 = 0.f, z1 = 0.f;
-                if (live) sample_depths(a, r, s, z0, off0, z1);
-                const float zj = z0 + off0;
-                float w;
+                float d1[32];
+                tc::wgmma_fence();
                 {
-                    float o16[16], o8[8];
-                    tc::tmem_ld16(d2_col + lane_sel + 32, o16);
-                    tc::tmem_ld8(d2_col + lane_sel + 48, o8);
-                    float sigma = (((P.written >> 3) & 1u) ? o8[3] : 0.f) + b2s[51];
-                    if (a.noise != nullptr && live) sigma += a.noise_std * a.noise[r.sample_base + s];
-                    const float delta = (s + 1 < S) ? (z1 - zj) * r.dnorm : 1e10f;
-                    const float dens = (a.clamp_mode == IDE3D_CLAMP_SOFTPLUS) ? softplus_precise(sigma) : fmaxf(sigma, 0.f);
-                    const float alpha = live ? 1.f - expf(-delta * dens) : 0.f;
-                    const float keep = live ? (1.f - alpha + 1e-10f) : 1.f;
-                    // exclusive product over the 8 samples of the ray in sample order, times the transmittance carried in
-                    float tr = T_in, mine = T_in;
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const float kj = __shfl_sync(kFull, keep, seg0 + j);
-                        if (j == d) mine = tr;
-                        tr *= kj;
+                    const uint64_t wh = wh0 + (B.w1_off >> 4), wl = wl0 + (B.w1_off >> 4);
+                    const int ks0 = B.k0 >> 4, ks1 = ks0 + (B.kcount >> 4);
+                    for (int ks = ks0; ks < ks1; ++ks) {
+                        const uint64_t off = (uint64_t)(ks * 2);               // 16 bf16 = 32 bytes along K, same column in A and W1
+                        tc::Wgmma<64>::ss(d1, ah0 + off, wh + off, ks > ks0);
+                        tc::Wgmma<64>::ss(d1, ah0 + off, wl + off, 1);
+                        tc::Wgmma<64>::ss(d1, al0 + off, wh + off, 1);
                     }
-                    T_in = tr;
-                    w = alpha * mine;
-                    acc_w += w;
-                    if (a.last_back && step == a.tiles_per_unit - 1) {
-                        float ws = acc_w;
-                        ws += __shfl_xor_sync(kFull, ws, 1); ws += __shfl_xor_sync(kFull, ws, 2); ws += __shfl_xor_sync(kFull, ws, 4);
-                        if (s == S - 1) w += 1.f - ws;
+                }
+                tc::wgmma_commit();
+                tc::wgmma_wait<0>();
+                tc::fence_regs(d1);
+                uint32_t ah[4][4], al[4][4];
+                const float* bb = b1s + b * 64;
+#pragma unroll
+                for (int ks = 0; ks < 4; ++ks)
+#pragma unroll
+                    for (int q = 0; q < 4; ++q) {                              // q: (n8 tile 2ks + q/2, row g + 8 (q%2))
+                        const int j = 2 * ks + (q >> 1), e = 4 * j + 2 * (q & 1);
+                        const float h0 = softplus2(d1[e] + bb[8 * j + 2 * c]);
+                        const float h1 = softplus2(d1[e + 1] + bb[8 * j + 2 * c + 1]);
+                        tc::split2_bf16(h0, h1, ah[ks][q], al[ks][q]);
                     }
-                    if (a.out_weights != nullptr && live) a.out_weights[r.sample_base + s] = w;
-                    acc_d = fmaf(w, zj, acc_d);
-#pragma unroll
-                    for (int c = 0; c < 16; ++c) acc[32 + c] = fmaf(w, (((P.written >> 2) & 1u) ? o16[c] : 0.f) + b2s[32 + c], acc[32 + c]);
-#pragma unroll
-                    for (int c = 0; c < 3; ++c) acc[48 + c] = fmaf(w, (((P.written >> 3) & 1u) ? o8[c] : 0.f) + b2s[48 + c], acc[48 + c]);
-                }
-                // ---- colour features (D2 columns 0..31)
-#pragma unroll
-                for (int c16 = 0; c16 < 2; ++c16) {
-                    float o16[16];
-                    tc::tmem_ld16(d2_col + lane_sel + c16 * 16, o16);
-#pragma unroll
-                    for (int c = 0; c < 16; ++c)
-                        acc[c16 * 16 + c] = fmaf(w, (((P.written >> c16) & 1u) ? o16[c] : 0.f) + b2s[c16 * 16 + c], acc[c16 * 16 + c]);
-                }
-                tc::tc_fence_before();                   // D2 reads ordered before the a2 arrival that lets layer 2 of the next tile overwrite it
+                tc::wgmma_fence();
+                const uint64_t wh = wh0 + (B.w2_off >> 4), wl = wl0 + (B.w2_off >> 4);
+                layer2_cols(B.w2_row0, B.w2_rows, d2, ah, al, wh, wl);
+                tc::wgmma_commit();
+                tc::wgmma_wait<0>();
+                tc::fence_regs(d2);
+                fence_frag(ah);
+                fence_frag(al);
             }
 
-            // ---- per-ray reduction over the 8 depth lanes and store (weights_sum is the sum BEFORE the last_back correction,
-            //      volumetric_rendering.py:56-72)
-            float wsum = acc_w, depth = acc_d;
+            // ---- sigma (column 51 = n8 tile 6, lane c == 1, second element), compositing weights of this lane's two samples
+            const float sig_row[2] = {__shfl_sync(kFull, d2[25], (lane & ~3) | 1), __shfl_sync(kFull, d2[27], (lane & ~3) | 1)};
+            const int s = step * kTileDepth + g;
 #pragma unroll
-            for (int m = 1; m < 8; m <<= 1) { wsum += __shfl_xor_sync(kFull, wsum, m); depth += __shfl_xor_sync(kFull, depth, m); }
+            for (int r = 0; r < 2; ++r) {
+                const RaySetup& R = r ? rB : rA;
+                const bool live = R.ok && (s < S);
+                float z0 = 0.f, off0 = 0.f, z1 = 0.f;
+                if (live) sample_depths(a, R, s, z0, off0, z1);
+                const float zj = z0 + off0;
+                float sigma = sig_row[r] + b2s[kOut - 1];
+                if (a.noise != nullptr && live) sigma += a.noise_std * a.noise[R.sample_base + s];
+                const float delta = (s + 1 < S) ? (z1 - zj) * R.dnorm : 1e10f;
+                const float dens = (a.clamp_mode == IDE3D_CLAMP_SOFTPLUS) ? softplus_precise(sigma) : fmaxf(sigma, 0.f);
+                const float alpha = live ? 1.f - expf(-delta * dens) : 0.f;
+                const float keep = live ? (1.f - alpha + 1e-10f) : 1.f;
+                // exclusive product over the 8 samples of the ray in sample order, times the transmittance carried in
+                float tr = T_in[r], mine = T_in[r];
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const float kj = __shfl_sync(kFull, keep, 4 * j + c);
+                    if (j == g) mine = tr;
+                    tr *= kj;
+                }
+                T_in[r] = tr;
+                float wt = alpha * mine;
+                acc_w[r] += wt;
+                if (a.last_back && step == a.tiles_per_unit - 1) {
+                    float ws = acc_w[r];
+                    ws += __shfl_xor_sync(kFull, ws, 4); ws += __shfl_xor_sync(kFull, ws, 8); ws += __shfl_xor_sync(kFull, ws, 16);
+                    if (s == S - 1) wt += 1.f - ws;
+                }
+                if (a.out_weights != nullptr && live && c == 0) a.out_weights[R.sample_base + s] = wt;
+                acc_d[r] = fmaf(wt, zj, acc_d[r]);
+#pragma unroll
+                for (int j = 0; j < 8; ++j)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int col = 8 * j + 2 * c + e;
+                        if (col < kOut - 1) acc[r][2 * j + e] = fmaf(wt, d2[4 * j + 2 * r + e] + b2s[col], acc[r][2 * j + e]);
+                    }
+            }
+        }
+
+        // ---- per-ray reduction over the 8 depth lanes and store (weights_sum is the sum BEFORE the last_back correction,
+        //      volumetric_rendering.py:56-72)
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const RaySetup& R = r ? rB : rA;
+            float wsum = acc_w[r], depth = acc_d[r];
+#pragma unroll
+            for (int m = 4; m < 32; m <<= 1) { wsum += __shfl_xor_sync(kFull, wsum, m); depth += __shfl_xor_sync(kFull, depth, m); }
             if (a.max_depth != 0.f) depth += (1.f - wsum) * a.max_depth;
-            const long long ray_index = (long long)r.n * (a.res_w * a.res_h) + r.ray;
+            const long long ray_index = (long long)R.n * (a.res_w * a.res_h) + R.ray;
             float* of = a.out_feat + ray_index * (kOut - 1);
 #pragma unroll
-            for (int c = 0; c < kOut - 1; ++c) {
-                float v = acc[c];
-                v += __shfl_xor_sync(kFull, v, 1); v += __shfl_xor_sync(kFull, v, 2); v += __shfl_xor_sync(kFull, v, 4);
-                if (a.white_back) v += 1.f - wsum;
-                if (a.fill_weight) v = wsum;
-                if (r.ok && (c & 7) == d) of[c] = v;
-            }
-            if (r.ok && d == 0) a.out_depth[ray_index] = depth;
+            for (int j = 0; j < 8; ++j)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    float v = acc[r][2 * j + e];
+                    v += __shfl_xor_sync(kFull, v, 4); v += __shfl_xor_sync(kFull, v, 8); v += __shfl_xor_sync(kFull, v, 16);
+                    if (a.white_back) v += 1.f - wsum;
+                    if (a.fill_weight) v = wsum;
+                    const int col = 8 * j + 2 * c + e;
+                    if (R.ok && g == 0 && col < kOut - 1) of[col] = v;
+                }
+            if (R.ok && lane == 0) a.out_depth[ray_index] = depth;
         }
     }
-
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(tmem_base, kGroups * kGroupCols);
 }
-
-int launch_raymarch_tc3(const TcArgs& a, int teams, cudaStream_t st, bool& handled);     // raymarch_tc3.cu
 
 // entry used by ide3d_raymarch_fwd (raymarch.cu); IDE3D_UNSUPPORTED when this decoder / layout has no TC kernel
 int launch_raymarch_tc(const ide3d_raymarch_params* p, bool channels_last, cudaStream_t st) {
@@ -330,25 +306,14 @@ int launch_raymarch_tc(const ide3d_raymarch_params* p, bool channels_last, cudaS
     a.units_x = ceil_div(p->res_w, kUnitW); a.units_y = ceil_div(p->res_h, kUnitH);
     a.num_units = a.units_x * a.units_y * a.n;
     a.tiles_per_unit = ceil_div(p->num_steps, kTileDepth);
-    // tuning knob: gather instruction shape
-    a.ray_major = env_int("IDE3D_TC_RAY_MAJOR", 1, 0, 1);
-    const int teams = env_int("IDE3D_TC_TEAMS", 2, 2, kMaxTeams);
-    const int smem = 2 * a.prog.wpart + teams * kStageBytes + (kTcMaxBlocks * 64 + 64) * 4 + (2 * kMaxTeams + (2 + kTcMaxBlocks) * kGroups) * 8 + 16 + 1024;
-    int grid = sm_count();
-    if (grid * kGroups > a.num_units) grid = ceil_div(a.num_units, kGroups);
-    // decoders with a density head of their own take the kernel that composites inside the tensor core (raymarch_tc3.cu)
-    if (env_int("IDE3D_TC_V2", 0, 0, 1) == 0) {
-        bool handled = false;
-        const int rc3 = launch_raymarch_tc3(a, teams, st, handled);
-        if (handled) return rc3;
-    }
-    if (teams == 2) {
-        IDE3D_CUDA(cudaFuncSetAttribute(raymarch_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        raymarch_tc_kernel<2><<<grid, TcCfg<2>::kThreads, smem, st>>>(a);
-    } else {
-        IDE3D_CUDA(cudaFuncSetAttribute(raymarch_tc_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        raymarch_tc_kernel<3><<<grid, TcCfg<3>::kThreads, smem, st>>>(a);
-    }
+    const int smem = 2 * a.prog.wpart + kWarpgroups * kStageBytes + (kTcMaxBlocks * 64 + 64) * 4 + 1024;
+    IDE3D_CUDA(cudaFuncSetAttribute(raymarch_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    int per_sm = 1;
+    IDE3D_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, raymarch_tc_kernel, kTcThreads, smem));
+    if (per_sm < 1) per_sm = 1;
+    int grid = sm_count() * per_sm;
+    if (grid * kWarpgroups > a.num_units) grid = ceil_div(a.num_units, kWarpgroups);
+    raymarch_tc_kernel<<<grid, kTcThreads, smem, st>>>(a);
     IDE3D_CHECK_LAUNCH("raymarch_tc_kernel");
     return IDE3D_OK;
 }

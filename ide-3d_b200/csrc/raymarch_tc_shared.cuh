@@ -1,6 +1,5 @@
-// Pieces shared by the tensor-core ray-march kernels (raymarch_tc.cu: generic decoders; raymarch_tc3.cu: decoders with an isolated
-// density head): work decomposition, per-ray set-up, the producers' tri-plane gather into the swizzled A stages, and the host-side
-// hidden-block program.
+// Pieces shared by the tensor-core kernels (raymarch_tc.cu: the fused renderer; voxel_tc.cu: density queries): tile geometry,
+// per-ray set-up, the tri-plane gather that feeds the swizzled A tiles, and the host-side hidden-block program.
 #pragma once
 #include <stdlib.h>
 
@@ -9,40 +8,23 @@
 
 namespace ide3d {
 
-constexpr int kGroups = 2;
-constexpr int kConsumerWarps = 4 * kGroups;
-constexpr int kMaxTeams = 3;                                             // producer teams (template parameter TEAMS = 2 or 3); a team owns one
-                                                                         // A stage and refills it as soon as layer 1 has read it
+constexpr int kWarpgroups = 2;                                          // warpgroups per CTA; each marches its own units
+constexpr int kTcThreads = 128 * kWarpgroups;
 constexpr int kTcMaxBlocks = 3;
-constexpr int kTileBytes = 128 * 128;                                    // [128 rows x 64 bf16]
+constexpr int kTileBytes = 64 * 128;                                     // [64 rows x 64 bf16], one warpgroup's tile
 constexpr int kStageBytes = 2 * kTileBytes;                              // hi + lo
-constexpr int kGroupCols = 256;                                          // TMEM columns per group: D1 3 x 64, D2 64
-constexpr int kD2Col = 64 * kTcMaxBlocks;
-constexpr int kUnitW = 4, kUnitH = 4, kTileDepth = 8;
-// register split (setmaxnreg): TEAMS = 2: 512 threads x 128 at launch -> consumers release down to 120, producers grow to 136
-// (256 x 120 + 256 x 136 = 65536).  TEAMS = 3: 640 threads x 96 at launch is the whole register file already; nobody can grow
-// (a setmaxnreg.inc with nothing released blocks forever -- measured: the first round-2 build hung exactly there), so no split.
-template <int TEAMS> struct TcCfg {
-    static constexpr int kThreads = 32 * (kConsumerWarps + 4 * TEAMS);
-    static constexpr int kConsumerRegs = (TEAMS == 3) ? 96 : 120;
-    static constexpr int kProducerRegs = (TEAMS == 3) ? 96 : 136;
-    static constexpr int kBaseRegs = (TEAMS == 3) ? 96 : 128;           // what __launch_bounds__(kThreads, 1) compiles to
-};
+constexpr int kUnitW = 4, kUnitH = 2, kTileDepth = 8;                    // unit = 4 x 2 rays; tile = 8 depth samples of the unit
 
-struct TcRun { int n0, n, accum; };
 struct TcBlock {
     const float* w1; int w1_ld, k0, kcount;        // W1 rows of this hidden block; inputs land at A columns [k0, k0+kcount)
     const float* b1;
     const float* w2; int w2_ld, out0, outc;        // W2[out, hidden cols of this block]; rows feed outputs [out0, out0+outc)
     int w1_off;                                    // byte offset of the [64 x 64] W1 tile inside a weight part (shared by two 32-input blocks)
-    int w2_off, w2_row0;                           // byte offset of the W2 row block; its first row is output column w2_row0
-    int nruns;
-    TcRun runs[4];                                 // layer-2 MMAs: D2 columns [n0, n0+n), accumulate or overwrite
+    int w2_off, w2_row0, w2_rows;                  // byte offset of the W2 row block; it feeds output columns [w2_row0, w2_row0 + w2_rows)
 };
 struct TcProgram {
     int nblocks;
     TcBlock blk[kTcMaxBlocks];
-    unsigned written;                              // bit g: D2 columns [16g, 16g+16) are produced by some block
     int wpart;                                     // bytes of one weight part (hi or lo), multiple of 1024
 };
 
@@ -61,7 +43,6 @@ struct TcArgs {
     const float* noise;
     float *out_feat, *out_depth, *out_weights;
     int units_x, units_y, num_units, tiles_per_unit;
-    int ray_major;                                 // gather instruction = 4 depth-consecutive samples of one ray (1) or 4 x-adjacent rays (0)
 };
 
 // log2(1 + 2^t): the hidden softplus in base-2 units (log2e folded into W1 / b1, ln2 into W2 at set-up).  ex2 of the clamped
@@ -76,26 +57,6 @@ __device__ __forceinline__ float softplus2(float t) {
 __device__ __forceinline__ void tile_store_bf16(unsigned char* tile, int row, int k, __nv_bfloat16 v) {
     *reinterpret_cast<__nv_bfloat16*>(tile + tc::sw128_offset(row, k >> 3) + (k & 7) * 2) = v;
 }
-
-// ---------------------------------------------------------------------------------------------------------------------------
-// work decomposition shared by producers and consumers
-struct Schedule {
-    int cnt0, cnt1;          // units of the two groups of this CTA
-    int tiles0, tiles1;      // tiles of the two groups
-    int m;                   // tiles of the shorter group: sequence numbers below 2m alternate between the groups
-};
-__device__ __forceinline__ Schedule make_schedule(const TcArgs& a) {
-    Schedule s;
-    const int stride = kGroups * gridDim.x;
-    const int f0 = blockIdx.x * kGroups, f1 = f0 + 1;
-    s.cnt0 = (f0 < a.num_units) ? (a.num_units - f0 + stride - 1) / stride : 0;
-    s.cnt1 = (f1 < a.num_units) ? (a.num_units - f1 + stride - 1) / stride : 0;
-    s.tiles0 = s.cnt0 * a.tiles_per_unit;
-    s.tiles1 = s.cnt1 * a.tiles_per_unit;
-    s.m = min(s.tiles0, s.tiles1);                       // group 0 never has fewer units than group 1
-    return s;
-}
-__device__ __forceinline__ int seq_of(const Schedule& s, int g, int t) { return (t < s.m) ? 2 * t + g : 2 * s.m + (t - s.m); }
 
 // per-ray constants
 struct RaySetup {
@@ -177,41 +138,6 @@ __device__ __forceinline__ void gather12(const char* __restrict__ base, const Ax
 #undef IDE3D_BLEND
 }
 
-// both tri-planes of one sample in one batch: 24 LDG.128 in flight (the 2-team variant has the registers for it)
-__device__ __forceinline__ void gather24(const char* __restrict__ tb, const char* __restrict__ sb, const AxisTaps& X, const AxisTaps& Yr,
-                                         const AxisTaps& Yc, const AxisTaps& Z, float (&at)[4], float (&as)[4]) {
-    float4 v[12], u[12];
-#define IDE3D_LD(k, C, R)                                                                                         \
-    {                                                                                                             \
-        const unsigned o0 = R.lo + C.lo + k * (kFeat * 4), o1 = R.lo + C.hi + k * (kFeat * 4);                    \
-        const unsigned o2 = R.hi + C.lo + k * (kFeat * 4), o3 = R.hi + C.hi + k * (kFeat * 4);                    \
-        v[4 * k + 0] = ldg_at(tb, o0); v[4 * k + 1] = ldg_at(tb, o1); v[4 * k + 2] = ldg_at(tb, o2); v[4 * k + 3] = ldg_at(tb, o3); \
-        u[4 * k + 0] = ldg_at(sb, o0); u[4 * k + 1] = ldg_at(sb, o1); u[4 * k + 2] = ldg_at(sb, o2); u[4 * k + 3] = ldg_at(sb, o3); \
-    }
-    IDE3D_LD(0, X, Yr)
-    IDE3D_LD(1, Yc, Z)
-    IDE3D_LD(2, X, Z)
-#undef IDE3D_LD
-    at[0] = at[1] = at[2] = at[3] = 0.f;
-    as[0] = as[1] = as[2] = as[3] = 0.f;
-#define IDE3D_BLEND(k, C, R)                                                                                      \
-    {                                                                                                             \
-        const float w4[4] = {C.wlo * R.wlo, C.whi * R.wlo, C.wlo * R.whi, C.whi * R.whi};                         \
-        float p[4] = {0.f, 0.f, 0.f, 0.f}, r[4] = {0.f, 0.f, 0.f, 0.f};                                           \
-        _Pragma("unroll") for (int tap = 0; tap < 4; ++tap) {                                                     \
-            const float4 t4 = v[k * 4 + tap], s4 = u[k * 4 + tap];                                                \
-            const float w_ = w4[tap];                                                                             \
-            p[0] += t4.x * w_; p[1] += t4.y * w_; p[2] += t4.z * w_; p[3] += t4.w * w_;                           \
-            r[0] += s4.x * w_; r[1] += s4.y * w_; r[2] += s4.z * w_; r[3] += s4.w * w_;                           \
-        }                                                                                                         \
-        _Pragma("unroll") for (int j = 0; j < 4; ++j) { at[j] += p[j]; as[j] += r[j]; }                           \
-    }
-    IDE3D_BLEND(0, X, Yr)
-    IDE3D_BLEND(1, Yc, Z)
-    IDE3D_BLEND(2, X, Z)
-#undef IDE3D_BLEND
-}
-
 __device__ __forceinline__ AxisTaps shfl_taps(const AxisTaps& t, int src) {
     AxisTaps r;
     r.lo = __shfl_sync(kFull, t.lo, src); r.hi = __shfl_sync(kFull, t.hi, src);
@@ -220,170 +146,10 @@ __device__ __forceinline__ AxisTaps shfl_taps(const AxisTaps& t, int src) {
 }
 
 
-// ---------------------------------------------------------------------------------------------------------------------------
-// producer warps (both kernels): a team of four warps fills one 32 KB A stage (a tile of 128 samples) at a time
-template <int TEAMS>
-__device__ __forceinline__ void producer_loop(const TcArgs& a, const Schedule& sch, unsigned char* stage_base, uint64_t* bar_full,
-                                              uint64_t* bar_empty, int pw, int lane) {
-    constexpr int kStages = TEAMS, kTeams = TEAMS;
-    const int S = a.steps;
-    const int unit_stride = kGroups * gridDim.x;
-    const int team = pw >> 2, qw = pw & 3;
-    const int total = sch.tiles0 + sch.tiles1;
-    const int shb = (int)(a.tex.sh * 4), swb = (int)(a.tex.sw * 4);     // strides in bytes (32-bit: checked by the launcher)
-    const int W = a.tex.w, H = a.tex.h;
-    const int q4 = lane & 7, grp = lane >> 3;
-    for (int seq = team; seq < total; seq += kTeams) {
-        int g, t;
-        if (seq < 2 * sch.m) { g = seq & 1; t = seq >> 1; } else { g = 0; t = sch.m + (seq - 2 * sch.m); }
-        const int ui = t / a.tiles_per_unit, step = t - ui * a.tiles_per_unit;
-        const int unit = blockIdx.x * kGroups + g + ui * unit_stride;
-        const RaySetup r = ray_setup(a, unit, lane >> 3, qw);
-        const int s = step * kTileDepth + (lane & 7);
-        const bool live = r.ok && (s < S);
-        float cx = 4.f, cy = 4.f, cz = 4.f;                                // far outside the planes: every tap gets weight 0
-        if (live) {
-            const float* M = a.cam2world + r.n * 16;
-            float z0, off0, z1;
-            sample_depths(a, r, s, z0, off0, z1);
-            const float pcx = r.dx * z0 + off0 * r.dx, pcy = r.dy * z0 + off0 * r.dy, pcz = r.dz * z0 + off0 * r.dz;
-            cx = (M[0] * pcx + M[1] * pcy + M[2] * pcz + M[3]) * a.box_scale;
-            cy = (M[4] * pcx + M[5] * pcy + M[6] * pcz + M[7]) * a.box_scale;
-            cz = (M[8] * pcx + M[9] * pcy + M[10] * pcz + M[11]) * a.box_scale;
-        }
-        // bilinear footprint per axis role, computed ONCE per sample by its own lane (dnnlib/util.py:589-596: plane 0 = (x,y),
-        // plane 1 = (y,z), plane 2 = (x,z)); the 8 lanes that fetch a sample's texels receive it by shuffle
-        const AxisFoot fx = axis_foot(cx, W), fyr = axis_foot(cy, H), fyc = axis_foot(cy, W), fz = axis_foot(cz, H);
-        const AxisTaps mX = axis_taps(fx.i0, fx.f, W, swb), mYr = axis_taps(fyr.i0, fyr.f, H, shb);
-        const AxisTaps mYc = axis_taps(fyc.i0, fyc.f, W, swb), mZ = axis_taps(fz.i0, fz.f, H, shb);
-        const char* tb = reinterpret_cast<const char*>(a.tex.base + (long long)r.n * a.tex.sn);
-        const char* sb = reinterpret_cast<const char*>(a.seg.base + (long long)r.n * a.seg.sn);
-
-        const int stage = seq % kStages, use = seq / kStages;
-        unsigned char* a_hi = stage_base + stage * kStageBytes;
-        unsigned char* a_lo = a_hi + kTileBytes;
-#pragma unroll 1
-        for (int it = 0; it < 8; ++it) {
-            const int src = a.ray_major ? (it * 4 + grp) : (grp * 8 + it);
-            AxisTaps X = shfl_taps(mX, src), Yc = shfl_taps(mYc, src);
-            const AxisTaps Yr = shfl_taps(mYr, src), Z = shfl_taps(mZ, src);
-            X.lo += q4 * 16; X.hi += q4 * 16; Yc.lo += q4 * 16; Yc.hi += q4 * 16;      // this lane's channel quad (every tap has one column role)
-            const int row = qw * 32 + src;
-            const uint32_t o_tex = tc::sw128_offset(row, q4 >> 1) + (q4 & 1) * 8;
-            const uint32_t o_seg = tc::sw128_offset(row, 4 + (q4 >> 1)) + (q4 & 1) * 8;
-            float f[4], f2[4];
-            uint2 hi, lo;
-            if constexpr (TEAMS == 2) gather24(tb, sb, X, Yr, Yc, Z, f, f2);    // 24 loads in flight per lane
-            else gather12(tb, X, Yr, Yc, Z, f);                                  // 12, then the shape tri-plane below
-            tc::split4_bf16(f, hi, lo);
-            // the stage is needed only now: the first gather of the tile overlaps the wait for layer 1 of the tile that used it before
-            if (it == 0) tc::mbar_wait(&bar_empty[stage], (use + 1) & 1);       // first use passes immediately
-            *reinterpret_cast<uint2*>(a_hi + o_tex) = hi;
-            *reinterpret_cast<uint2*>(a_lo + o_tex) = lo;
-            if constexpr (TEAMS != 2) gather12(sb, X, Yr, Yc, Z, f2);
-            tc::split4_bf16(f2, hi, lo);
-            *reinterpret_cast<uint2*>(a_hi + o_seg) = hi;
-            *reinterpret_cast<uint2*>(a_lo + o_seg) = lo;
-        }
-        tc::fence_async_smem();                                            // my generic-proxy stores -> async proxy (UMMA)
-        __syncwarp();
-        if (lane == 0) tc::mbar_arrive(&bar_full[stage]);
-    }
-}
-
-// Cooperative variant (raymarch_tc3.cu): ALL eight producer warps fill the same tile -- warp pw takes 16 rows (two pixel columns x 8
-// depth samples of pixel row pw / 2) -- so one tile is in production at a time: half the per-tile latency and half the L1 working
-// set of two independent teams.  `stages` A buffers (2 or 3) are cycled in tile-sequence order; bar_full counts 8 arrivals.
-__device__ __forceinline__ void prefetch_l1(const char* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
-
-__device__ __forceinline__ void producer_loop_coop(const TcArgs& a, const Schedule& sch, unsigned char* stage_base, uint64_t* bar_full,
-                                                   uint64_t* bar_empty, int pw, int lane, int stages, int prefetch) {
-    const int S = a.steps;
-    const int unit_stride = kGroups * gridDim.x;
-    const int total = sch.tiles0 + sch.tiles1;
-    const int shb = (int)(a.tex.sh * 4), swb = (int)(a.tex.sw * 4);
-    const int W = a.tex.w, H = a.tex.h;
-    const int q4 = lane & 7, grp = lane >> 3;
-    const int prow = pw >> 1, half = pw & 1;                                 // pixel row of the unit, which pair of pixel columns
-    const int l16 = lane & 15;                                               // lanes 16..31 mirror 0..15 (same sample)
-    // position (plane grid units) and frame of this lane's sample in tile `seq`
-    auto sample_of = [&](int seq, int& n, float& cx, float& cy, float& cz) {
-        int g, t;
-        if (seq < 2 * sch.m) { g = seq & 1; t = seq >> 1; } else { g = 0; t = sch.m + (seq - 2 * sch.m); }
-        const int ui = t / a.tiles_per_unit, step = t - ui * a.tiles_per_unit;
-        const int unit = blockIdx.x * kGroups + g + ui * unit_stride;
-        const RaySetup r = ray_setup(a, unit, half * 2 + (l16 >> 3), prow);
-        const int s = step * kTileDepth + (l16 & 7);
-        n = r.n;
-        cx = cy = cz = 4.f;                                                   // far outside the planes: every tap gets weight 0
-        if (r.ok && s < S) {
-            const float* M = a.cam2world + r.n * 16;
-            float z0, off0, z1;
-            sample_depths(a, r, s, z0, off0, z1);
-            const float pcx = r.dx * z0 + off0 * r.dx, pcy = r.dy * z0 + off0 * r.dy, pcz = r.dz * z0 + off0 * r.dz;
-            cx = (M[0] * pcx + M[1] * pcy + M[2] * pcz + M[3]) * a.box_scale;
-            cy = (M[4] * pcx + M[5] * pcy + M[6] * pcz + M[7]) * a.box_scale;
-            cz = (M[8] * pcx + M[9] * pcy + M[10] * pcz + M[11]) * a.box_scale;
-        }
-    };
-    int stage = 0, use = 0;
-    for (int seq = 0; seq < total; ++seq) {
-        int n;
-        float cx, cy, cz;
-        sample_of(seq, n, cx, cy, cz);
-        const AxisFoot fx = axis_foot(cx, W), fyr = axis_foot(cy, H), fyc = axis_foot(cy, W), fz = axis_foot(cz, H);
-        const AxisTaps mX = axis_taps(fx.i0, fx.f, W, swb), mYr = axis_taps(fyr.i0, fyr.f, H, shb);
-        const AxisTaps mYc = axis_taps(fyc.i0, fyc.f, W, swb), mZ = axis_taps(fz.i0, fz.f, H, shb);
-        const char* tb = reinterpret_cast<const char*>(a.tex.base + (long long)n * a.tex.sn);
-        const char* sb = reinterpret_cast<const char*>(a.seg.base + (long long)n * a.seg.sn);
-        if (prefetch && seq + 1 < total) {
-            // the NEXT tile's texel lines into L1 while this tile is gathered: each lane owns one sample of it; lanes 0-15 prefetch its
-            // 12 lines of the texture tri-plane, lanes 16-31 the 12 lines of the shape tri-plane (one 128-byte line per tap)
-            int n2;
-            float px, py, pz;
-            sample_of(seq + 1, n2, px, py, pz);
-            const AxisFoot gx = axis_foot(px, W), gyr = axis_foot(py, H), gyc = axis_foot(py, W), gz = axis_foot(pz, H);
-            const AxisTaps pX = axis_taps(gx.i0, gx.f, W, swb), pYr = axis_taps(gyr.i0, gyr.f, H, shb);
-            const AxisTaps pYc = axis_taps(gyc.i0, gyc.f, W, swb), pZ = axis_taps(gz.i0, gz.f, H, shb);
-            const char* pb = reinterpret_cast<const char*>(((lane < 16) ? a.tex.base : a.seg.base) + (long long)n2 * a.tex.sn);
-            prefetch_l1(pb + pYr.lo + pX.lo); prefetch_l1(pb + pYr.lo + pX.hi); prefetch_l1(pb + pYr.hi + pX.lo); prefetch_l1(pb + pYr.hi + pX.hi);
-            prefetch_l1(pb + pZ.lo + pYc.lo + 128); prefetch_l1(pb + pZ.lo + pYc.hi + 128); prefetch_l1(pb + pZ.hi + pYc.lo + 128); prefetch_l1(pb + pZ.hi + pYc.hi + 128);
-            prefetch_l1(pb + pZ.lo + pX.lo + 256); prefetch_l1(pb + pZ.lo + pX.hi + 256); prefetch_l1(pb + pZ.hi + pX.lo + 256); prefetch_l1(pb + pZ.hi + pX.hi + 256);
-        }
-        unsigned char* a_hi = stage_base + stage * kStageBytes;
-        unsigned char* a_lo = a_hi + kTileBytes;
-#pragma unroll 1
-        for (int it = 0; it < 4; ++it) {
-            const int src = it * 4 + grp;                                     // 4 depth-consecutive samples of one ray per instruction
-            AxisTaps X = shfl_taps(mX, src), Yc = shfl_taps(mYc, src);
-            const AxisTaps Yr = shfl_taps(mYr, src), Z = shfl_taps(mZ, src);
-            X.lo += q4 * 16; X.hi += q4 * 16; Yc.lo += q4 * 16; Yc.hi += q4 * 16;
-            const int row = prow * 32 + half * 16 + src;
-            const uint32_t o_tex = tc::sw128_offset(row, q4 >> 1) + (q4 & 1) * 8;
-            const uint32_t o_seg = tc::sw128_offset(row, 4 + (q4 >> 1)) + (q4 & 1) * 8;
-            float f[4], f2[4];
-            uint2 hi, lo;
-            gather24(tb, sb, X, Yr, Yc, Z, f, f2);
-            tc::split4_bf16(f, hi, lo);
-            if (it == 0) tc::mbar_wait(&bar_empty[stage], (use + 1) & 1);     // first use passes immediately
-            *reinterpret_cast<uint2*>(a_hi + o_tex) = hi;
-            *reinterpret_cast<uint2*>(a_lo + o_tex) = lo;
-            tc::split4_bf16(f2, hi, lo);
-            *reinterpret_cast<uint2*>(a_hi + o_seg) = hi;
-            *reinterpret_cast<uint2*>(a_lo + o_seg) = lo;
-        }
-        tc::fence_async_smem();
-        __syncwarp();
-        if (lane == 0) tc::mbar_arrive(&bar_full[stage]);
-        if (++stage == stages) { stage = 0; ++use; }
-    }
-}
-
 // Build the hidden-block program from the head list and lay the weight tiles out compactly.  Returns false when the decoder does
 // not fit (hidden not a multiple of 64, more than kTcMaxBlocks blocks, outputs beyond 64 columns).
 inline bool build_program(const ide3d_decoder& d, TcProgram& P) {
     P.nblocks = 0;
-    P.written = 0;
     for (int h = 0; h < d.num_heads; ++h) {
         const ide3d_mlp_head& H = d.heads[h];
         if (H.hidden <= 0 || H.hidden % 64 != 0) return false;
@@ -398,19 +164,10 @@ inline bool build_program(const ide3d_decoder& d, TcProgram& P) {
             B.b1 = H.b1 + c * 64;
             B.w2 = H.w2 + c * 64; B.w2_ld = H.hidden;
             B.out0 = H.out_offset; B.outc = H.out_count;
-            // layer-2 column range in units of 16, split into runs of equal "already written" status
+            // layer-2 column range in units of 16 (an N of 16..64 for the layer-2 MMA)
             const int g0 = H.out_offset / 16, g1 = (H.out_offset + H.out_count + 15) / 16;
             B.w2_row0 = g0 * 16;
-            B.nruns = 0;
-            int gi = g0;
-            while (gi < g1) {
-                const int st = (P.written >> gi) & 1;
-                int ge = gi + 1;
-                while (ge < g1 && (int)((P.written >> ge) & 1) == st) ++ge;
-                B.runs[B.nruns++] = TcRun{gi * 16, (ge - gi) * 16, st};
-                gi = ge;
-            }
-            for (int q = g0; q < g1; ++q) P.written |= 1u << q;
+            B.w2_rows = (g1 - g0) * 16;
         }
     }
     if (P.nblocks == 0) return false;
@@ -431,22 +188,11 @@ inline bool build_program(const ide3d_decoder& d, TcProgram& P) {
     int off = ntiles * 64 * 128;
     for (int b = 0; b < P.nblocks; ++b) {
         TcBlock& B = P.blk[b];
-        const int rows = ((B.out0 + B.outc + 15) / 16) * 16 - B.w2_row0;
         B.w2_off = off;
-        off += rows * 128;
+        off += B.w2_rows * 128;
     }
     P.wpart = (off + 1023) & ~1023;
     return true;
 }
-
-// Tuning knobs (IDE3D_TC_*) exist only in a build made with -DIDE3D_TUNING (IDE3D_BUILD_TUNING=1 python ide-3d_b200/build.py), which is
-// what scripts/bench_raymarch.py's A/B runs use; the product build always takes the defaults.
-inline int env_int(const char* name, int dflt, int lo, int hi) {
-    const char* v = tuning_env(name);
-    if (!v) return dflt;
-    const int x = atoi(v);
-    return (x < lo || x > hi) ? dflt : x;
-}
-
 
 }  // namespace ide3d

@@ -2,7 +2,7 @@
 //
 // The reference evaluates, per modulated convolution, `styles = affine(w)` (FullyConnectedLayer, inversion/networks.py:136-165,
 // :476) and `dcoefs = rsqrt(sum_{i,k} (W[o,i,k] s[n,i])^2 + 1e-8)` (:89-90); with 18 layers that was ~150 tiny library launches
-// per step (addmm / square / sum / rsqrt / mul; profiles/r01_launches_bench_steady_state_v2.txt: 10 % of the step).  Both are
+// per step (addmm / square / sum / rsqrt / mul; about 10 % of the step in the first measured profile).  Both are
 // independent of the activations, so they are computed up front:
 //   styles[l][n, i] = ((A_l[i, :] . ws[n, w_index_l, :]) * w_gain_l + b_l[i] * b_gain_l) * out_scale_l        (one warp per row i)
 //   dcoefs[l][n, o] = rsqrt(sum_i styles[l][n, i]^2 * Wsq_l[o, i] + 1e-8),  Wsq_l[o, i] = sum_k W_l[o, i, k]^2   (one warp per o)

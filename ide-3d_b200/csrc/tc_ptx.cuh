@@ -1,6 +1,7 @@
-// Thin inline-PTX wrappers for the Blackwell (sm_100a) tensor-core path: tcgen05.{alloc,mma,commit,ld,fence},
-// mbarrier, proxy fences, shared-memory matrix descriptors.  Bit layouts follow the PTX ISA "tcgen05" chapter
-// (instruction descriptor, shared-memory descriptor) as used by CUTLASS' cute::UMMA.
+// Thin inline-PTX wrappers for the Hopper (sm_90a) tensor-core path: warpgroup MMA (wgmma.mma_async with the A operand in
+// shared memory or in registers, fp32 accumulators in registers), its fences, proxy fences, named barriers and the shared-memory
+// matrix descriptor.  Bit layouts follow the PTX ISA "wgmma" chapter (matrix descriptor, register fragments) as used by CUTLASS'
+// cute::GMMA.
 #pragma once
 
 #include <cuda_bf16.h>
@@ -11,114 +12,33 @@ namespace tc {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// ---------------------------------------------------------------------------------------- mbarrier
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ uint32_t mbar_try_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t"
-        "}\n"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    return ok;
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    while (!mbar_try_wait(bar, parity)) {}      // (a __nanosleep back-off here measured 5% slower)
-}
-
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}\n" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// register re-partitioning between warpgroups (all 128 threads of the warpgroup execute it)
-template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
-template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
-
-// ---------------------------------------------------------------------------------------- fences
-// generic-proxy shared-memory writes -> visible to the async proxy (tensor core operand reads)
+// ---------------------------------------------------------------------------------------- fences / barriers
+// generic-proxy shared-memory writes -> visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 // named barrier over `threads` threads (id 1..15; 0 is __syncthreads)
 __device__ __forceinline__ void bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
-// ---------------------------------------------------------------------------------------- TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {   // one full warp; ncols power of 2 >= 32
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {     // same warp that allocated
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp receives lane (taddr.lane + i)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// wgmma ordering: fence before the first MMA that touches accumulator / A registers written by ordinary instructions;
+// commit closes a group of MMAs; wait_group<N> returns when at most N groups are still in flight
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// the accumulators are written asynchronously: keep the compiler from moving their reads across the wait
+template <int R> __device__ __forceinline__ void fence_regs(float (&d)[R]) {
 #pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-
-// narrower shapes of the same access (thread i <-> lane taddr.lane + i, N consecutive columns); loads wait for completion
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float (&v)[8]) {
-    uint32_t r[8];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];\n"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-// registers -> TMEM: thread i writes lane taddr.lane + i, 8 consecutive 32-bit columns (16 packed bf16 = one K step of an A operand)
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&r)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};\n" ::"r"(taddr), "r"(r[0]), "r"(r[1]),
-                 "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------------------- descriptors
-// Instruction descriptor, kind::f16 with BF16 operands, FP32 accumulate, both operands K-major.
-//   [4,6) D format (1 = F32)  [7,10) A format (1 = BF16)  [10,13) B format (1 = BF16)
-//   [15] A major (0 = K)  [16] B major (0 = K)  [17,23) N >> 3  [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
 // Shared-memory matrix descriptor for a K-major operand stored as 128-byte rows with the 128B swizzle
 // (8-row x 128-byte atoms, 16-byte chunks XORed with row % 8; atoms 1024 bytes apart along M/N):
-//   [0,14) start address >> 4   [16,30) leading byte offset >> 4 (unused for swizzled K-major)
-//   [32,46) stride byte offset >> 4 (1024 B between 8-row groups)   [46,48) version = 1   [61,64) layout = 2 (SWIZZLE_128B)
+//   [0,14) start address >> 4   [16,30) leading byte offset >> 4 (unused for swizzled K-major: 1)
+//   [32,46) stride byte offset >> 4 (1024 B between 8-row groups)   [49,52) base offset (0: atoms 1024-byte aligned)
+//   [62,64) layout = 1 (SWIZZLE_128B)
+// Moving along K inside the 128-byte row: + (bytes >> 4) on the start address.
 __device__ __forceinline__ uint64_t make_sdesc_sw128(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(1024u >> 4) << 32) | (1ull << 46) | (2ull << 61);
+    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024u >> 4) << 32) | (1ull << 62);
 }
 
 // byte offset of 16-byte chunk `c` (0..7) of row `r` inside a swizzle-128B tile
@@ -126,33 +46,87 @@ __device__ __forceinline__ uint32_t sw128_offset(int r, int c) {
     return (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + (((c ^ r) & 7) << 4));
 }
 
-// D[tmem] (+)= A[smem] * B[smem]^T, one UMMA (M = 128, K = 16 bf16), issued by ONE thread
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
+// ---------------------------------------------------------------------------------------- warpgroup MMA, M = 64, K = 16 bf16
+// Issued by all 128 threads of a warpgroup.  Accumulator fragment of thread t (warp w = t / 32, lane l): rows 16w + l/4 and
+// 16w + l/4 + 8, columns 8j + 2(l%4) + {0, 1}: d[4j + 0..1] (first row), d[4j + 2..3] (second row).  The register A fragment of a
+// K = 16 step has the same row / column ownership: a[0] = (row, k 2(l%4)..+1), a[1] = (row + 8, same k), a[2] / a[3] = k + 8.
+template <int N> struct Wgmma;
 
-// same with the A operand in TMEM ("TS" form): lane = row m, 32-bit column c holds K elements 2c (low half) and 2c+1 (high half);
-// one K = 16 step is 8 columns starting at a_tmem
-__device__ __forceinline__ void umma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-        "}\n" ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
+template <> struct Wgmma<16> {
+    // D[64 x 16] (+)= A[smem] . B[smem]^T
+    __device__ __forceinline__ static void ss(float* d, uint64_t a_desc, uint64_t b_desc, int scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+            : "l"(a_desc), "l"(b_desc), "r"(scale_d));
+    }
+    // D[64 x 16] += A[registers] . B[smem]^T
+    __device__ __forceinline__ static void rs(float* d, const uint32_t (&a)[4], uint64_t b_desc) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 0;\n\t}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(1));
+    }
+};
 
-// all previously issued MMAs of this thread arrive on `bar` when they have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
+template <> struct Wgmma<32> {
+    // D[64 x 32] (+)= A[smem] . B[smem]^T
+    __device__ __forceinline__ static void ss(float* d, uint64_t a_desc, uint64_t b_desc, int scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "l"(a_desc), "l"(b_desc), "r"(scale_d));
+    }
+    // D[64 x 32] += A[registers] . B[smem]^T
+    __device__ __forceinline__ static void rs(float* d, const uint32_t (&a)[4], uint64_t b_desc) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(1));
+    }
+};
+
+template <> struct Wgmma<48> {
+    // D[64 x 48] (+)= A[smem] . B[smem]^T
+    __device__ __forceinline__ static void ss(float* d, uint64_t a_desc, uint64_t b_desc, int scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, 0, 0;\n\t}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+            : "l"(a_desc), "l"(b_desc), "r"(scale_d));
+    }
+    // D[64 x 48] += A[registers] . B[smem]^T
+    __device__ __forceinline__ static void rs(float* d, const uint32_t (&a)[4], uint64_t b_desc) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %29, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, {%24, %25, %26, %27}, %28, p, 1, 1, 0;\n\t}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(1));
+    }
+};
+
+template <> struct Wgmma<64> {
+    // D[64 x 64] (+)= A[smem] . B[smem]^T
+    __device__ __forceinline__ static void ss(float* d, uint64_t a_desc, uint64_t b_desc, int scale_d) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "l"(a_desc), "l"(b_desc), "r"(scale_d));
+    }
+    // D[64 x 64] += A[registers] . B[smem]^T
+    __device__ __forceinline__ static void rs(float* d, const uint32_t (&a)[4], uint64_t b_desc) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(1));
+    }
+};
 
 // fp32 -> (hi, lo) bf16 pair with hi + lo ~= x to 16 mantissa bits
 __device__ __forceinline__ void split_bf16(float x, __nv_bfloat16& hi, __nv_bfloat16& lo) {
@@ -168,8 +142,13 @@ __device__ __forceinline__ void split4_bf16(const float (&f)[4], uint2& hi, uint
     hi = make_uint2(*reinterpret_cast<const uint32_t*>(&h01), *reinterpret_cast<const uint32_t*>(&h23));
     lo = make_uint2(*reinterpret_cast<const uint32_t*>(&l01), *reinterpret_cast<const uint32_t*>(&l23));
 }
-__device__ __forceinline__ uint32_t pack_bf16(__nv_bfloat16 a, __nv_bfloat16 b) {
-    return (uint32_t)__bfloat16_as_ushort(a) | ((uint32_t)__bfloat16_as_ushort(b) << 16);
+// two fp32 -> one packed bf16 hi pair and one lo pair
+__device__ __forceinline__ void split2_bf16(float x0, float x1, uint32_t& hi, uint32_t& lo) {
+    const __nv_bfloat162 h = __floats2bfloat162_rn(x0, x1);
+    const float2 b = __bfloat1622float2(h);
+    const __nv_bfloat162 l = __floats2bfloat162_rn(x0 - b.x, x1 - b.y);
+    hi = *reinterpret_cast<const uint32_t*>(&h);
+    lo = *reinterpret_cast<const uint32_t*>(&l);
 }
 
 }  // namespace tc

@@ -1,4 +1,4 @@
-// upfirdn2d for sm_100a: pad -> zero-upsample -> FIR -> decimate.
+// upfirdn2d for sm_90a: pad -> zero-upsample -> FIR -> decimate.
 // Replaces upfirdn2d_kernel_small/_large (torch_utils/ops/upfirdn2d.cu:29-200) behind the field set of
 // upfirdn2d_kernel_params (upfirdn2d.h:14-40).
 //
@@ -236,7 +236,7 @@ struct TmaGeom {
     using AX = Axis<UX, DX, FW, PHX>;
     using AY = Axis<UY, DY, FH, PHY>;
     // The innermost box coordinate has to sit on a 16-byte boundary: UTMALDG raises "illegal instruction" for x = -1 or 31
-    // (fp32) while x = 0 or 64 work (scripts/tma_probe.cu, profiles/r01_tma_probe.txt).  The box therefore starts at the
+    // (fp32) while x = 0 or 64 work.  The box therefore starts at the
     // 16-byte aligned column at or left of the tile origin and is up to kVec-1 columns wider; the window base is shifted.
     static constexpr int kVec = 16 / (int)sizeof(T);
     static constexpr int BW = (AX::kTileIn + kVec - 1 + kVec - 1) / kVec * kVec, BH = AY::kTileIn;
@@ -482,8 +482,8 @@ __device__ __forceinline__ void cl_patch_body(const UpfirArgs& p, const float (&
             for (int c = 0; c < 4; ++c) acc[a][b][c] = 0.f;
     if (p.add != nullptr) {
         // skip-connection form (upsample2d(img) + y + b): the accumulators START from the new contribution, so its 16 loads are in
-        // flight together with the window loads instead of after the FIR (the kernel is latency bound: long-scoreboard 11.7 per issue at
-        // 46 % of the HBM peak, profiles/r02p_ncu_step_fir_epilogue_kernels.txt) -- same registers, twice the loads in flight
+        // flight together with the window loads instead of after the FIR (the kernel is latency bound) -- same registers, twice the
+        // loads in flight
         const T* ain = (const T*)p.add + n * p.asn + cv * 4;
         float bv[4] = {0.f, 0.f, 0.f, 0.f};
         if (p.bias != nullptr) V4<T>::ld((const T*)p.bias + cv * 4, bv);

@@ -1,21 +1,17 @@
-// Density queries on the tensor cores: sigma for 128 points per tile (extract_shapes.py:99-150, the 256^3 grid of config 4, and
-// renderer.sample_voxel(..., sigma_only) with explicit points), for decoders whose density head reads the shape planes alone
-// (the generator's three-head decoder).  The machinery of raymarch_tc3.cu without the march:
-//   producers (2 teams x 4 warps)  point -> 3 x 4 bilinear taps of the SHAPE tri-plane only (8 lanes x LDG.128 per texel), blend,
-//                                  bf16 hi / lo, swizzled A stage (columns 32..63 of the [128 x 64] tile)
-//   issuer (one lane per group)    D1[128 x 64] = A . W1_sigma^T, three bf16 products per K step; two D1 slots per group, so layer 1 of
-//                                  tile t+1 runs while the consumers are still on tile t
-//   consumers (2 groups x 4 warps) tcgen05.ld -> + b1 -> softplus -> 64 -> 1 second layer as 64 FFMA per point -> + b2 -> out
+// Density queries on the tensor cores: sigma for 64 points per warpgroup tile (extract_shapes.py:99-150, the 256^3 grid of config 4,
+// and renderer.sample_voxel(..., sigma_only) with explicit points), for decoders whose density head reads the shape planes alone
+// (the generator's three-head decoder).  The machinery of raymarch_tc.cu without the march:
+//   gather   every warp: its 16 points -> 3 x 4 bilinear taps of the SHAPE tri-plane only (8 lanes x LDG.128 per texel), blend,
+//            bf16 hi / lo, swizzled A tile (columns 32..63 of the [64 x 64] tile)
+//   layer 1  D1[64 x 64] = A . W1_sigma^T, wgmma (both operands in shared memory), three bf16 products per K step
+//   epilog   + b1 -> softplus -> 64 -> 1 second layer as FFMA over the lane's 16 hidden columns, 4-lane reduction -> + b2 -> out
 // No per-point intermediate touches HBM; the only global traffic is the texel gather (L1 / L2 hits for a coherent grid) and 4 bytes
-// out per point.  The CUDA-core kernel of voxel.cu (255 registers, 2112 FFMA per point) remains for every other decoder / layout.
+// out per point.  The CUDA-core kernel of voxel.cu remains for every other decoder / layout.
 #include "raymarch_tc_shared.cuh"
 
 namespace ide3d {
 namespace vtc {
 
-constexpr int kTeams = 2, kStages = 2;
-constexpr int kThreads = 32 * (kConsumerWarps + 4 * kTeams + 4);           // 640
-constexpr int kBaseRegs = 96, kIssuerRegs = 40, kConsumerRegs = 88, kProducerRegs = 128;
 constexpr int kW1Bytes = 64 * 128;                                           // [64 hidden x 64 K] bf16, K columns 32..63 used
 
 struct Args {
@@ -45,34 +41,17 @@ __device__ __forceinline__ void grid_point(const Args& a, long long idx, float& 
     z = __fmul_rn(__fadd_rn(__fmul_rn(s2, a.voxel_size), a.org_x), a.pre_scale);
 }
 
-struct Sched { long long cnt[2]; long long m; };
-__device__ __forceinline__ long long seq_of(const Sched& s, int g, long long t) { return (t < s.m) ? 2 * t + g : 2 * s.m + (t - s.m); }
-
-__device__ __forceinline__ float4 lds4(uint32_t addr) {
-    float4 v;
-    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-    return v;
-}
-__device__ __forceinline__ float ex2f(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-__device__ __forceinline__ float lg2f(float x) { float y; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-
-__global__ void __launch_bounds__(kThreads, 1) sigma_tc_kernel(const Args a) {
+__global__ void __launch_bounds__(kTcThreads) sigma_tc_kernel(const Args a) {
     extern __shared__ unsigned char smem_raw[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     unsigned char* w_hi = smem;
     unsigned char* w_lo = smem + kW1Bytes;
-    unsigned char* stage_base = smem + 2 * kW1Bytes;
-    unsigned char* misc = stage_base + kStages * kStageBytes;
-    float* b1s = reinterpret_cast<float*>(misc);                          // [64] x log2e
-    float* wsig = b1s + 64;                                                // [64] x ln2
-    uint64_t* bar_full = reinterpret_cast<uint64_t*>(wsig + 64);         // [kStages]
-    uint64_t* bar_empty = bar_full + kStages;                             // [kStages]
-    uint64_t* bar_d1 = bar_empty + kStages;                               // [kGroups][2]
-    uint64_t* bar_free = bar_d1 + kGroups * 2;                            // [kGroups][2]  (4 arrivals)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_free + kGroups * 2);
+    unsigned char* tile_base = smem + 2 * kW1Bytes;
+    float* b1s = reinterpret_cast<float*>(tile_base + kWarpgroups * kStageBytes);     // [64] x log2e
+    float* wsig = b1s + 64;                                                            // [64] x ln2
 
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    for (int i = tid; i < 64 * 32; i += kThreads) {
+    const int tid = threadIdx.x, lane = tid & 31;
+    for (int i = tid; i < 64 * 32; i += kTcThreads) {
         const int j = i >> 5, k = i & 31;
         __nv_bfloat16 hi, lo;
         tc::split_bf16(a.w1[j * 32 + k] * 1.4426950408889634f, hi, lo);
@@ -80,68 +59,26 @@ __global__ void __launch_bounds__(kThreads, 1) sigma_tc_kernel(const Args a) {
         tile_store_bf16(w_lo, j, 32 + k, lo);
     }
     if (tid < 64) { b1s[tid] = a.b1[tid] * 1.4426950408889634f; wsig[tid] = a.w2[tid] * 0.6931471805599453f; }
-    if (tid == 0) {
-        for (int i = 0; i < kStages; ++i) { tc::mbar_init(&bar_full[i], 4); tc::mbar_init(&bar_empty[i], 1); }
-        for (int i = 0; i < kGroups * 2; ++i) { tc::mbar_init(&bar_d1[i], 1); tc::mbar_init(&bar_free[i], 4); }
-        tc::fence_mbar_init();
-    }
-    if (warp == 0) tc::tmem_alloc(tmem_slot, 256);
     tc::fence_async_smem();
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    // tiles of this CTA: group g takes tiles blockIdx.x*2 + g + k * 2 * gridDim.x
-    const long long stride = (long long)kGroups * gridDim.x;
-    Sched sch;
-    for (int g = 0; g < 2; ++g) {
-        const long long f = (long long)blockIdx.x * kGroups + g;
-        sch.cnt[g] = (f < a.num_tiles) ? (a.num_tiles - f + stride - 1) / stride : 0;
-    }
-    sch.m = min(sch.cnt[0], sch.cnt[1]);
-    constexpr int kFirstProducer = kConsumerWarps, kFirstIssuer = kConsumerWarps + 4 * kTeams;
+    const int wg = tid >> 7, w = (tid >> 5) & 3;
+    const int g = lane >> 2, c = lane & 3;
+    const int q4 = lane & 7, grp = lane >> 3, l16 = lane & 15;
+    const int shb = (int)(a.seg.sh * 4), swb = (int)(a.seg.sw * 4);
+    const int W = a.seg.w, H = a.seg.h;
+    unsigned char* a_hi = tile_base + wg * kStageBytes;
+    unsigned char* a_lo = a_hi + kTileBytes;
+    const uint64_t ah = tc::make_sdesc_sw128(tc::smem_u32(a_hi)), al = tc::make_sdesc_sw128(tc::smem_u32(a_lo));
+    const uint64_t wh = tc::make_sdesc_sw128(tc::smem_u32(w_hi)), wl = tc::make_sdesc_sw128(tc::smem_u32(w_lo));
+    const float sig_b = a.b2[0];
+    const long long stride = (long long)kWarpgroups * gridDim.x;
 
-    if (warp >= kFirstIssuer) {
-        // =========================================================================== MMA issuers
-        tc::setmaxnreg_dec<kIssuerRegs>();
-        const int g = warp - kFirstIssuer;
-        if (g < kGroups && lane == 0 && sch.cnt[g] > 0) {
-            const uint32_t d1_col = tmem_base + g * 128;
-            const uint32_t stage_u = tc::smem_u32(stage_base);
-            const uint64_t wh = tc::make_sdesc_sw128(tc::smem_u32(w_hi)), wl = tc::make_sdesc_sw128(tc::smem_u32(w_lo));
-            const uint32_t idesc = tc::make_idesc_bf16(128, 64);
-            for (long long t = 0; t < sch.cnt[g]; ++t) {
-                const long long seq = seq_of(sch, g, t);
-                const int stage = (int)(seq % kStages), slot = (int)(t & 1);
-                if (t >= 2) tc::mbar_wait(&bar_free[g * 2 + slot], (uint32_t)(((t - 2) >> 1) & 1));     // tile t-2 has been read out of this slot
-                tc::mbar_wait(&bar_full[stage], (uint32_t)((seq / kStages) & 1));
-                tc::tc_fence_after();
-                const uint64_t ah = tc::make_sdesc_sw128(stage_u + stage * kStageBytes), al = ah + (kTileBytes >> 4);
-#pragma unroll
-                for (int ks = 2; ks < 4; ++ks) {                                     // K columns 32..63 (the shape features)
-                    tc::umma_bf16(d1_col + slot * 64, ah + ks * 2, wh + ks * 2, idesc, ks > 2);
-                    tc::umma_bf16(d1_col + slot * 64, ah + ks * 2, wl + ks * 2, idesc, 1);
-                    tc::umma_bf16(d1_col + slot * 64, al + ks * 2, wh + ks * 2, idesc, 1);
-                }
-                tc::umma_commit(&bar_d1[g * 2 + slot]);
-                tc::umma_commit(&bar_empty[stage]);
-            }
-        }
-    } else if (warp >= kFirstProducer) {
-        // =========================================================================== producers
-        tc::setmaxnreg_inc<kProducerRegs>();
-        const int pw = warp - kFirstProducer, team = pw >> 2, qw = pw & 3;
-        const long long total = sch.cnt[0] + sch.cnt[1];
-        const int shb = (int)(a.seg.sh * 4), swb = (int)(a.seg.sw * 4);
-        const int W = a.seg.w, H = a.seg.h;
-        const int q4 = lane & 7, grp = lane >> 3;
-        for (long long seq = team; seq < total; seq += kTeams) {
-            int g; long long t;
-            if (seq < 2 * sch.m) { g = (int)(seq & 1); t = seq >> 1; } else { g = (sch.cnt[0] > sch.cnt[1]) ? 0 : 1; t = sch.m + (seq - 2 * sch.m); }
-            const long long tile = (long long)blockIdx.x * kGroups + g + t * stride;
-            const int n = (int)(tile / a.tiles_per_item);
-            const long long p = (tile - (long long)n * a.tiles_per_item) * 128 + qw * 32 + lane;
+    for (long long tile = (long long)blockIdx.x * kWarpgroups + wg; tile < a.num_tiles; tile += stride) {
+        const int n = (int)(tile / a.tiles_per_item);
+        const long long p0 = (tile - (long long)n * a.tiles_per_item) * 64 + w * 16;       // first point of this warp's 16 rows
+        {
+            const long long p = p0 + l16;
             float cx = 4.f, cy = 4.f, cz = 4.f;
             if (p < a.P) {
                 if (a.grid_mode) grid_point(a, a.first + p, cx, cy, cz);
@@ -152,78 +89,52 @@ __global__ void __launch_bounds__(kThreads, 1) sigma_tc_kernel(const Args a) {
             const AxisTaps mX = axis_taps(fx.i0, fx.f, W, swb), mYr = axis_taps(fyr.i0, fyr.f, H, shb);
             const AxisTaps mYc = axis_taps(fyc.i0, fyc.f, W, swb), mZ = axis_taps(fz.i0, fz.f, H, shb);
             const char* sb = reinterpret_cast<const char*>(a.seg.base + (long long)n * a.seg.sn);
-            const int stage = (int)(seq % kStages);
-            const long long use = seq / kStages;
-            unsigned char* a_hi = stage_base + stage * kStageBytes;
-            unsigned char* a_lo = a_hi + kTileBytes;
 #pragma unroll 1
-            for (int it = 0; it < 8; ++it) {
+            for (int it = 0; it < 4; ++it) {
                 const int src = it * 4 + grp;
                 AxisTaps X = shfl_taps(mX, src), Yc = shfl_taps(mYc, src);
                 const AxisTaps Yr = shfl_taps(mYr, src), Z = shfl_taps(mZ, src);
                 X.lo += q4 * 16; X.hi += q4 * 16; Yc.lo += q4 * 16; Yc.hi += q4 * 16;
-                const int row = qw * 32 + src;
-                const uint32_t o_seg = tc::sw128_offset(row, 4 + (q4 >> 1)) + (q4 & 1) * 8;
+                const uint32_t o_seg = tc::sw128_offset(w * 16 + src, 4 + (q4 >> 1)) + (q4 & 1) * 8;
                 float f[4];
                 uint2 hi, lo;
                 gather12(sb, X, Yr, Yc, Z, f);
                 tc::split4_bf16(f, hi, lo);
-                if (it == 0) tc::mbar_wait(&bar_empty[stage], (uint32_t)((use + 1) & 1));
+                if (it == 0) tc::bar_sync(1 + wg, 128);                        // every warp is past the MMAs of the previous tile
                 *reinterpret_cast<uint2*>(a_hi + o_seg) = hi;
                 *reinterpret_cast<uint2*>(a_lo + o_seg) = lo;
             }
             tc::fence_async_smem();
-            __syncwarp();
-            if (lane == 0) tc::mbar_arrive(&bar_full[stage]);
+            tc::bar_sync(1 + wg, 128);
         }
-    } else {
-        // =========================================================================== consumers
-        tc::setmaxnreg_dec<kConsumerRegs>();
-        const int g = warp >> 2, qw = warp & 3;
-        const uint32_t d1_col = tmem_base + g * 128;
-        const uint32_t lane_sel = (uint32_t)(qw * 32) << 16;
-        const uint32_t b1_u = tc::smem_u32(b1s), wsig_u = tc::smem_u32(wsig);
-        const float sig_b = a.b2[0];
-        for (long long t = 0; t < sch.cnt[g]; ++t) {
-            const int slot = (int)(t & 1);
-            tc::mbar_wait(&bar_d1[g * 2 + slot], (uint32_t)((t >> 1) & 1));
-            tc::tc_fence_after();
-            float sig = 0.f;
+        float d1[32];
+        tc::wgmma_fence();
 #pragma unroll
-            for (int c16 = 0; c16 < 4; ++c16) {
-                float v[16], e[16];
-                tc::tmem_ld16(d1_col + slot * 64 + c16 * 16 + lane_sel, v);
-                if (c16 == 3) {
-                    tc::tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) tc::mbar_arrive(&bar_free[g * 2 + slot]);
-                }
+        for (int ks = 2; ks < 4; ++ks) {                                       // K columns 32..63 (the shape features)
+            tc::Wgmma<64>::ss(d1, ah + ks * 2, wh + ks * 2, ks > 2);
+            tc::Wgmma<64>::ss(d1, ah + ks * 2, wl + ks * 2, 1);
+            tc::Wgmma<64>::ss(d1, al + ks * 2, wh + ks * 2, 1);
+        }
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::fence_regs(d1);
+        float sig[2] = {0.f, 0.f};                                             // rows g and g + 8
 #pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const float4 b = lds4(b1_u + (c16 * 16 + q * 4) * 4);
-                    v[4 * q] += b.x; v[4 * q + 1] += b.y; v[4 * q + 2] += b.z; v[4 * q + 3] += b.w;
-                }
+        for (int j = 0; j < 8; ++j)
 #pragma unroll
-                for (int i = 0; i < 16; ++i) e[i] = ex2f(fminf(v[i], 126.f));
+            for (int e = 0; e < 2; ++e) {
+                const int col = 8 * j + 2 * c + e;
 #pragma unroll
-                for (int i = 0; i < 16; ++i) e[i] = lg2f(1.f + e[i]);
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const float4 ws = lds4(wsig_u + (c16 * 16 + q * 4) * 4);
-                    sig = fmaf(fmaxf(e[4 * q], v[4 * q]), ws.x, sig); sig = fmaf(fmaxf(e[4 * q + 1], v[4 * q + 1]), ws.y, sig);
-                    sig = fmaf(fmaxf(e[4 * q + 2], v[4 * q + 2]), ws.z, sig); sig = fmaf(fmaxf(e[4 * q + 3], v[4 * q + 3]), ws.w, sig);
-                }
+                for (int r = 0; r < 2; ++r) sig[r] = fmaf(softplus2(d1[4 * j + 2 * r + e] + b1s[col]), wsig[col], sig[r]);
             }
-            const long long tile = (long long)blockIdx.x * kGroups + g + t * stride;
-            const int n = (int)(tile / a.tiles_per_item);
-            const long long p = (tile - (long long)n * a.tiles_per_item) * 128 + qw * 32 + lane;
-            if (p < a.P) a.out[(long long)n * a.P + p] = sig + sig_b;
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            float v = sig[r];
+            v += __shfl_xor_sync(kFull, v, 1); v += __shfl_xor_sync(kFull, v, 2);
+            const long long p = p0 + g + 8 * r;
+            if (c == 0 && p < a.P) a.out[(long long)n * a.P + p] = v + sig_b;
         }
     }
-
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(tmem_base, 256);
 }
 
 }  // namespace vtc
@@ -252,13 +163,16 @@ int launch_sigma_tc(const ide3d_triplane& seg, const ide3d_decoder& dec, const f
     a.points = points; a.P = P; a.n = n; a.box_scale = box_scale; a.out = out;
     a.grid_mode = grid_mode; a.grid_n = grid_n; a.voxel_size = voxel_size; a.org_x = org_x; a.org_y = org_y; a.org_z = org_z;
     a.pre_scale = pre_scale; a.first = first;
-    a.tiles_per_item = (P + 127) / 128;
+    a.tiles_per_item = (P + 63) / 64;
     a.num_tiles = a.tiles_per_item * n;
-    const int smem = 2 * vtc::kW1Bytes + vtc::kStages * kStageBytes + 128 * 4 + (2 * vtc::kStages + 4 * kGroups) * 8 + 16 + 1024;
-    long long grid = sm_count();
-    if (grid * kGroups > a.num_tiles) grid = (a.num_tiles + kGroups - 1) / kGroups;
+    const int smem = 2 * vtc::kW1Bytes + kWarpgroups * kStageBytes + 128 * 4 + 1024;
     IDE3D_CUDA(cudaFuncSetAttribute(vtc::sigma_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    vtc::sigma_tc_kernel<<<(unsigned)grid, vtc::kThreads, smem, st>>>(a);
+    int per_sm = 1;
+    IDE3D_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, vtc::sigma_tc_kernel, kTcThreads, smem));
+    if (per_sm < 1) per_sm = 1;
+    long long grid = (long long)sm_count() * per_sm;
+    if (grid * kWarpgroups > a.num_tiles) grid = (a.num_tiles + kWarpgroups - 1) / kWarpgroups;
+    vtc::sigma_tc_kernel<<<(unsigned)grid, kTcThreads, smem, st>>>(a);
     IDE3D_CHECK_LAUNCH("sigma_tc_kernel");
     return IDE3D_OK;
 }

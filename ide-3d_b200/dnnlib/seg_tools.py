@@ -1,5 +1,5 @@
 """Semantic-mask helpers of the reference's dnnlib/seg_tools.py that sit right after the renderer (SURVEY.md §8f rank 4):
-`COLOR_MAP` (:13-32) and `mask2color` (:75-82) -- argmax over the 19 semantic logits + colour look-up -- as ONE sm_100a pass
+`COLOR_MAP` (:13-32) and `mask2color` (:75-82) -- argmax over the 19 semantic logits + colour look-up -- as ONE sm_90a pass
 (ide3d_mask2color) instead of an argmax, a zero-fill and 19 masked assignments.  CUDA tensors only, like every op here."""
 
 import ctypes as C

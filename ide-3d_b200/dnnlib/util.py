@@ -1,4 +1,4 @@
-"""Network helpers of the reference's dnnlib/util.py (:561-617) on the sm_100a gather kernel.
+"""Network helpers of the reference's dnnlib/util.py (:561-617) on the sm_90a gather kernel.
 
     sample_from_triplane(coordinates [N,P,3], grid [N,96,H,W]) -> [N*P, 32]   (:580-599)
     sample_from_2dgrid(coordinates [N,P,2], grid [N,C,H,W])    -> [N*P, C]     (:603-617)

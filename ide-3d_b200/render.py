@@ -68,7 +68,7 @@ def raymarch(planes_tex, planes_seg, decoder, cam2world, resolution=(64, 64), nu
     """Fused render of N frames.  -> feat [N,R,51], depth [N,R,1], weights [N,R,S,1] | None.
     jitter_u: explicit uniforms [N,R,S]; jitter_seed: in-kernel counter hash; neither: no jitter.
     z_vals: explicit sample depths [N,R,S] ascending along S (replaces linspace + jitter; num_steps is taken from it).
-    precision: 'auto' | 'fp32' (CUDA-core FFMA decoder) | 'tc' (tcgen05 decoder, bf16x3 products).
+    precision: 'auto' | 'fp32' (CUDA-core FFMA decoder) | 'tc' (wgmma tensor-core decoder, bf16x3 products).
     Differentiable w.r.t. the planes, the camera and the decoder parameters (when `decoder` is a list of heads holding the
     live parameters): the forward is the same fused kernel, the backward is render_grad.RaymarchFunction."""
     kw = dict(resolution=resolution, num_steps=num_steps, fov=fov, ray_start=ray_start, ray_end=ray_end, box_scale=box_scale,

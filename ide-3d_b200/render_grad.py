@@ -1,7 +1,7 @@
 """Backward of the fused renderer (SURVEY.md §8f rank 1: PTI / encoder callers differentiate through G.synthesis,
 inversion/training/projectors/w_plus_projector_ide3d.py:115).
 
-Round-1 form: the FORWARD is always the fused sm_100a kernel (render.raymarch); the BACKWARD re-evaluates the same chain
+Round-1 form: the FORWARD is always the fused sm_90a kernel (render.raymarch); the BACKWARD re-evaluates the same chain
 -- rays (volumetric_rendering.py:77-97), jitter (:99-105), cam2world (:122-134), tri-plane gather (dnnlib/util.py:580-617,
 grid_sample_gradfix.py:26-29), decoder heads, compositing (:34-74) -- with differentiable torch library ops on the GPU and
 lets autograd produce the gradients w.r.t. the planes, the decoder parameters and the camera.  That costs the memory the

@@ -1,4 +1,4 @@
-"""Fused bias + activation (+ gain, clamp) on sm_100a.
+"""Fused bias + activation (+ gain, clamp) on sm_90a.
 
 Same public surface as the reference's torch_utils/ops/bias_act.py: `activation_funcs` (:21-31) and
 `bias_act(x, b=None, dim=1, act='linear', alpha=None, gain=None, clamp=None, impl='cuda')` (:52).
@@ -135,7 +135,7 @@ def bias_act(x, b=None, dim=1, act='linear', alpha=None, gain=None, clamp=None, 
 def scaled_bias_act(x, scale=None, noise=None, b=None, act='linear', alpha=None, gain=None, clamp=None, next_scale=None,
                     only_next=False):
     """Extension: ``bias_act(fma(x, scale[:, :, None, None], noise), b, act=...)`` -- the tail of an activation-scaled
-    modulated convolution (inversion/networks.py:104-105 then :512) -- as ONE sm_100a pass when nothing needs a gradient;
+    modulated convolution (inversion/networks.py:104-105 then :512) -- as ONE sm_90a pass when nothing needs a gradient;
     otherwise exactly that composition of the two reference ops (so autograd behaves as in the reference).
     x [N,C,H,W]; scale [N,C] (demodulation coefficients) | None; noise broadcastable [.,1,H,W] | None; b [C] | None.
     next_scale [N,C]: additionally return ``y * next_scale[:, :, None, None]`` (the style modulation that opens the next

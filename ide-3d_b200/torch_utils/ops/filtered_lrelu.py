@@ -1,4 +1,4 @@
-"""Filtered leaky ReLU on sm_100a: bias -> up-FIR -> gain*lrelu*clamp -> down-FIR.
+"""Filtered leaky ReLU on sm_90a: bias -> up-FIR -> gain*lrelu*clamp -> down-FIR.
 
 Public surface of the reference's torch_utils/ops/filtered_lrelu.py:56 `filtered_lrelu(x, fu, fd, b, up, down,
 padding, gain, slope, clamp, flip_filter, impl)`.  The fused plugin call returns `return_code = -1` when it has

@@ -1,4 +1,4 @@
-"""upfirdn2d family on sm_100a: pad -> zero-upsample -> FIR -> decimate.
+"""upfirdn2d family on sm_90a: pad -> zero-upsample -> FIR -> decimate.
 
 Public surface of the reference's torch_utils/ops/upfirdn2d.py: `setup_filter` (:70), `upfirdn2d` (:118),
 `filter2d` (:277), `upsample2d` (:313), `downsample2d` (:352) -- same arguments and semantics.  Compute

@@ -6,7 +6,7 @@ the nearest in-repo definitions are in inversion/networks.py (modulated_conv2d :
 The classes below restate those layers for inference: same parameter names/shapes/initialisation and the same
 arithmetic, with the StyleNeRF-only options (pixelshuffle / liif / 3-D modes, magnitude EMA, ...) left out.
 Every convolution goes to cuDNN (conv2d_resample -> conv2d_gradfix); the surrounding ops are this package's
-sm_100a kernels: upfirdn2d (FIR after the transposed conv, skip-image upsampling) and bias_act.
+sm_90a kernels: upfirdn2d (FIR after the transposed conv, skip-image upsampling) and bias_act.
 """
 
 import os
@@ -20,9 +20,9 @@ from ..torch_utils.ops import bias_act, conv2d_resample, fma, upfirdn2d
 
 FUSED_MODCONV_MIN_RES = 1 << 30      # block resolutions >= this use the grouped (weight-modulated) convolution
 
-# B200 layout choice: activations of every block are channels_last (NHWC) regardless of dtype.  The tf32 / fp16 tensor-core
+# Layout choice: activations of every block are channels_last (NHWC) regardless of dtype.  The tf32 / fp16 tensor-core
 # convolutions cuDNN picks are NHWC kernels -- with NCHW tensors it brackets every convolution with nchwToNhwc / nhwcToNchw
-# passes (14 % of the step, profiles/r01_launches_bench_steady_state_final.txt) -- and the renderer gathers NHWC tri-planes
+# passes -- and the renderer gathers NHWC tri-planes
 # anyway.  The reference only does this for its fp16 layers (inversion/networks.py:746).  IDE3D_CHANNELS_LAST=0 restores
 # the reference's NCHW fp32 layout (same values).
 CHANNELS_LAST = os.environ.get('IDE3D_CHANNELS_LAST', '1') != '0'
@@ -30,7 +30,7 @@ STYLE_PLAN = os.environ.get('IDE3D_STYLE_PLAN', '1') != '0'      # styles + demo
 CHAIN_MODULATION = True              # epilogues also write the next layer's `x * styles` (SynthesisBlock._features)
 # 1x1 convolutions of NHWC activations as one [N*H*W, I] x [I, O] matrix product (cuBLASLt, tf32 exactly when the cuDNN convolution
 # it replaces would use tf32) instead of cuDNN's conv3d_fprop kernels, which stream these shapes at ~40 % of the HBM peak.
-# Measured on B200 (round 1): the step gets SLOWER with it (7.76 vs 7.35 ms), so it stays off; kept as a switch for the record.
+# Off by default; kept as a switch for A/B runs.
 CONV1X1_AS_MATMUL = os.environ.get('IDE3D_CONV1X1_MM', '0') != '0'
 
 
@@ -321,7 +321,7 @@ class SynthesisBlock(torch.nn.Module):
             fused_modconv = (not self.training) and (dtype == torch.float32 or int(ws.shape[0]) == 1)
             # Scaling activations instead of weights keeps the convolution a plain batched one (the grouped per-sample
             # form is what the reference uses in eval, inversion/networks.py:802; both are the same arithmetic up to
-            # rounding) and is faster below FUSED_MODCONV_MIN_RES on B200 (measured, DESIGN.md).
+            # rounding); the grouped form is used from FUSED_MODCONV_MIN_RES up.
             thr = int(os.environ.get('IDE3D_FUSED_MODCONV_MIN_RES', FUSED_MODCONV_MIN_RES))
             fused_modconv = fused_modconv and self.resolution >= thr
         # Inference in fp32 with activation scaling: every epilogue also writes the next layer's `x * styles`, so the

@@ -51,7 +51,7 @@ class DecoderHead(torch.nn.Module):
 # ================================================================================================ renderer
 @persistence.persistent_class
 class TriPlaneRenderer(torch.nn.Module):
-    """Per-ray tri-plane sampling -> decoder -> alpha compositing, through the fused sm_100a kernels
+    """Per-ray tri-plane sampling -> decoder -> alpha compositing, through the fused sm_90a kernels
     (ide3d_b200.render)."""
 
     def __init__(self, hidden=64, box_warp=1.0):

@@ -1,5 +1,5 @@
 """Volume-rendering free functions with the reference's names and signatures
-(training/volumetric_rendering.py), computed by the sm_100a stage kernels in csrc/stages.cu.
+(training/volumetric_rendering.py), computed by the sm_90a stage kernels in csrc/stages.cu.
 
     fancy_integration          :34    -> ide3d_integrate
     get_initial_rays_trig      :77    -> ide3d_initial_rays

@@ -1,5 +1,5 @@
 /*
- * ide3d_b200 -- C-ABI of the B200-native IDE-3D hot path (libide3d_b200.so).
+ * ide3d_b200 -- C-ABI of the H100-native IDE-3D hot path (libide3d_b200.so).
  *
  * Drop-in boundary.  Every entry point below replaces one pybind11/Python boundary of the
  * reference (citations are relative to the reference tree, MrTornado24/IDE-3D @ b2ee653):
@@ -212,7 +212,7 @@ typedef struct ide3d_decoder {
 enum ide3d_jitter { IDE3D_JITTER_NONE = 0, IDE3D_JITTER_TENSOR = 1, IDE3D_JITTER_HASH = 2, IDE3D_JITTER_ZVALS = 3 };
 enum ide3d_clamp { IDE3D_CLAMP_SOFTPLUS = 0, IDE3D_CLAMP_RELU = 1 };
 /* AUTO: tensor cores when the decoder / layout allows, else CUDA cores.  FP32: CUDA-core FFMA, plain fp32.
- * TC: tcgen05 tensor cores, every product as bf16 hi*hi + hi*lo + lo*hi with fp32 accumulation (16-bit operand
+ * TC: wgmma tensor cores, every product as bf16 hi*hi + hi*lo + lo*hi with fp32 accumulation (16-bit operand
  * mantissas); IDE3D_UNSUPPORTED if the decoder shape or plane layout has no tensor-core kernel. */
 enum ide3d_precision { IDE3D_PRECISION_AUTO = 0, IDE3D_PRECISION_FP32 = 1, IDE3D_PRECISION_TC = 2 };
 

@@ -10,9 +10,9 @@ Pinning status
 --------------
 The reference repository ships **no tests and no golden vectors** (SURVEY.md §4, §8c), so the oracle
 is pinned the only way available: every function here was compared, in the build container, against
-the reference's own Python functions imported from ``/root/reference`` (``tests/golden/make_golden.py``)
+the reference's own Python functions imported from the reference tree (``tests/golden/make_golden.py``)
 and the resulting input/output tensors are committed under ``tests/golden/*.npz``.
-``tests/test_oracle_golden.py`` replays those fixtures on every run (no ``/root/reference`` needed).
+``tests/test_oracle_golden.py`` replays those fixtures on every run (no reference tree needed).
 
 What is NOT pinned by the reference ("parity unpinned" — the generator class that composes the
 free functions is absent from the reference tree, SURVEY.md §0): the decoder MLP widths, the

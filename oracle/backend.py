@@ -74,7 +74,7 @@ def _renderer_sample_voxel(self, img_v, seg_v, points, sigma_only=False):
 @contextlib.contextmanager
 def cpu_reference_ops(reference_layout=True):
     """Inside the context the product's op modules and renderer compute with the oracle on CPU tensors.
-    reference_layout: activations stay NCHW as in the reference's fp32 path (inversion/networks.py:746) -- the B200 build's
+    reference_layout: activations stay NCHW as in the reference's fp32 path (inversion/networks.py:746) -- the GPU build's
     NHWC choice is a GPU layout decision and would only slow the CPU arm down; False keeps whatever the product is set to."""
     from ide3d_b200.torch_utils.ops import bias_act as p_ba, filtered_lrelu as p_fl, upfirdn2d as p_up
     from ide3d_b200.training import networks as p_nw, triplane as p_tp

@@ -1,6 +1,6 @@
 """Oracle (test infrastructure): camera pose helpers restated from the reference.
 
-Follows /root/reference/training/volumetric_rendering.py
+Follows the reference's training/volumetric_rendering.py
   * sample_camera_positions   :147-193
   * create_cam2world_matrix   :195-213
   * LookAtPoseSampler.sample  :268-295

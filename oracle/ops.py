@@ -1,6 +1,6 @@
 """Oracle (test infrastructure): CPU restatement of the StyleGAN custom ops on the hot path.
 
-Follows (relative to /root/reference/torch_utils/ops):
+Follows (relative to the reference's torch_utils/ops):
   bias_act.py:91-120 (_bias_act_ref) and bias_act.cu:23-147 (gradient forms, clamp rule)
   upfirdn2d.py:70-115 (setup_filter), :167-211 (_upfirdn2d_ref), upfirdn2d.cpp:35-36 (output size)
   filtered_lrelu.py:121-153 (_filtered_lrelu_ref), filtered_lrelu.cpp:82-96 + filtered_lrelu.cu:494-505

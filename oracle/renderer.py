@@ -3,7 +3,7 @@
 torch-CPU fp32, written from the reference's Python functions (cited per function).  Used only as
 the checker for the CUDA kernels and as the CPU baseline leg of bench.py -- never shipped.
 
-Reference files followed (relative to /root/reference):
+Reference files followed (relative to the reference tree):
   training/volumetric_rendering.py   rays :77-97, jitter :99-105, world transform :108-136,
                                      compositing :34-74, importance pdf :224-265
   dnnlib/util.py                     tri-plane gather :580-617

@@ -20,7 +20,7 @@ def peak():
 
 
 def load_reference_ops():
-    """The reference's own torch_utils.ops wrappers on the reference's own CUDA plugins, prebuilt for sm_100a by
+    """The reference's own torch_utils.ops wrappers on the reference's own CUDA plugins, prebuilt for sm_90a by
     baseline/build_ref_plugins.py (custom_ops._cached_plugins is pre-seeded, so get_plugin returns them without a JIT build)."""
     import importlib.util
     ref = os.path.join(ROOT, 'baseline', '_ref')
@@ -91,7 +91,7 @@ def main():
                 gbs = nbytes / ms / 1e6
                 rec = {'op': name, 'dtype': str(dtype).replace('torch.', ''), 'layout': layout, 'shape': list(x.shape), 'out': list(y.shape),
                        'ours_ms': round(ms, 4), 'algorithmic_GB': round(nbytes / 1e9, 3), 'achieved_GBs': round(gbs, 1), 'peak_GBs': pk, 'frac': round(gbs / pk, 3)}
-                if refops is not None:              # the reference's own sm_100a-compiled plugin on the same tensor, same call
+                if refops is not None:              # the reference's own sm_90a-compiled plugin on the same tensor, same call
                     try:
                         with torch.no_grad():
                             rms, ry = timeit(lambda: fn(refops), reps=5, warm=2)

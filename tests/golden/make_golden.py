@@ -1,10 +1,9 @@
 #!/usr/bin/env python
 """Generate tests/golden/*.npz by running the REFERENCE's own Python functions (imported read-only
-from /root/reference) on small seeded inputs, and assert on the spot that oracle/ reproduces them.
+from the reference IDE-3D tree named by IDE3D_REFERENCE) on small seeded inputs, and assert on the spot that oracle/
+reproduces them:
 
-Run in the build container only (the GPU box has no /root/reference):
-
-    PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py
+    IDE3D_REFERENCE=/path/to/IDE-3D PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py
 
 The committed .npz files are the contract that tests/test_oracle_golden.py (CPU) and the -m gpu parity
 tests replay.  The reference ships no tests or golden vectors of its own (SURVEY.md §4), so these
@@ -19,7 +18,7 @@ import sys
 import numpy as np
 import torch
 
-REF = '/root/reference'
+REF = os.environ.get('IDE3D_REFERENCE', '')
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.dont_write_bytecode = True

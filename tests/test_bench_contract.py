@@ -1,5 +1,5 @@
 """bench.py's reference arm (`--impl reference`: the oracle port of the reference's CPU path, the one leg of the bench that runs without a
-GPU) prints ONE JSON line with the contract's keys; and the traffic citation file the GPU arm reads is well formed."""
+GPU) prints ONE JSON line with the contract's keys; and the GPU arm's roofline inputs are what it documents."""
 
 import json
 import os
@@ -25,11 +25,13 @@ def test_reference_arm_prints_one_contract_line():
     assert d['e2e'] == {'value': d['value'], 'unit': 'frames/s', 'h2d_bytes_per_step': 0, 'd2h_bytes_per_step': 0}
 
 
-def test_raymarch_traffic_citation():
+def test_roofline_inputs():
+    """Algorithmic bytes per frame: both tri-planes once + the 53 output floats per ray.  No measured DRAM-traffic capture of the
+    current ray-march kernel is committed, and the bench must say so instead of citing one."""
     import importlib.util
     spec = importlib.util.spec_from_file_location('bench_mod', os.path.join(ROOT, 'bench.py'))
     bench = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(bench)
     traffic, src = bench.raymarch_traffic()
-    assert traffic is not None and 1e8 < traffic < 1e9 and 'profiles/' in src
+    assert (traffic is None) == (not os.path.exists(bench.TRAFFIC_JSON)) and isinstance(src, str)
     assert bench.FRAME_ALGO_BYTES == 2 * 96 * 256 * 256 * 4 + 64 * 64 * 53 * 4

@@ -57,7 +57,8 @@ def test_shard_helpers():
 
 
 @pytest.mark.timeout(300)
-def test_two_rank_gloo_frame_and_slab_gather():
+def test_two_rank_gloo_frame_and_slab_gather(monkeypatch):
+    monkeypatch.setenv('CUDA_VISIBLE_DEVICES', '')        # a CPU test: the spawned ranks must not claim GPUs the machine may lack
     ctx = mp.get_context('spawn')
     q = ctx.Queue()
     port = 29500 + (os.getpid() % 2000)

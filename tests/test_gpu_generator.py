@@ -1,10 +1,9 @@
 """GPU parity of the WHOLE synthesis path: TriPlaneGenerator.synthesis on cuda (NHWC backbone, chained epilogues, TMA FIR,
-fused skip step, tcgen05 / fp32 ray-march, SR blocks) against the same module evaluated by the CPU oracle in the reference's
+fused skip step, tensor-core / fp32 ray-march, SR blocks) against the same module evaluated by the CPU oracle in the reference's
 layout (oracle.backend.cpu_reference_ops: NCHW, reference op chain).  cuDNN tf32 is switched off for the comparison so that
 the convolutions are fp32 on both sides.  Tolerances are relative to max|tensor| (2.5 ... 5.9 here): 1e-4 on the 128^2 image and
-semantic maps and on the 32^2 feature image, 2e-5 on depth, 1 uint8 level on the final frames.  Measured on B200 (round 1): image
-4.6e-5 absolute on a 5.9 range, feature image 2.2e-5, depth 2.9e-6, semantic maps 3.0e-5 -- identical for NHWC / NCHW, chained / unchained
-epilogues and the optional matmul form of the 1x1 convolutions."""
+semantic maps and on the 32^2 feature image, 2e-5 on depth, 1 uint8 level on the final frames -- the same for NHWC / NCHW, chained /
+unchained epilogues and the optional matmul form of the 1x1 convolutions."""
 
 import pytest
 import torch
@@ -64,7 +63,7 @@ def test_synthesis_on_gpu_matches_cpu_oracle(case, channels_last, chain, mm):
 @pytest.mark.parametrize('channels_last', [True, False])
 def test_blocks_on_gpu_reproduce_recorded_reference_classes(channels_last):
     """tests/golden/networks.npz (outputs of the reference's own MappingNetwork / SynthesisBlock / SegSynthesisBlock, see
-    tests/test_oracle_golden.py) replayed through the CUDA path: same state_dicts, sm_100a ops, fp32 convolutions."""
+    tests/test_oracle_golden.py) replayed through the CUDA path: same state_dicts, sm_90a ops, fp32 convolutions."""
     import numpy as np
     from conftest import load_golden
     from ide3d_b200.training import networks as nw
@@ -113,9 +112,9 @@ def test_stream_frames_matches_batch_loop_and_lands_in_pinned_host_memory(case):
         G.cpu()
     assert streamed.dtype == torch.uint8 and streamed.device.type == 'cpu' and streamed.is_pinned() and tuple(streamed.shape) == (4, 3, 128, 128)
     assert (streamed.int() - looped.cpu().int()).abs().max() <= 1            # batch 2 vs batch 4: cuDNN may pick different algorithms
-    # the two halves are the same inputs rendered as two batches of the same size: bit-identical (scripts/determinism.py on B200,
-    # profiles/r02a_parity_fullsize_and_determinism.txt: every stage is run-to-run bit-equal under all cudnn.benchmark /
-    # cudnn.deterministic settings; the one-level difference seen in round 1 came from comparing DIFFERENT batch sizes, above)
+    # the two halves are the same inputs rendered as two batches of the same size: bit-identical (scripts/determinism.py: every stage
+    # is run-to-run bit-equal under all cudnn.benchmark / cudnn.deterministic settings; a one-level difference comes only from
+    # comparing DIFFERENT batch sizes, above)
     assert torch.equal(streamed[:2], streamed[2:])
 
 

@@ -15,7 +15,7 @@ from oracle import camera as ocam, renderer as orr
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
 
-# Decoder precision modes of the fused kernel: 'fp32' = CUDA-core FFMA (plain fp32), 'tc' = tcgen05 tensor cores with
+# Decoder precision modes of the fused kernel: 'fp32' = CUDA-core FFMA (plain fp32), 'tc' = wgmma tensor cores with
 # every product evaluated as bf16 hi*hi + hi*lo + lo*hi and fp32 accumulation (operands carry 16 mantissa bits, i.e.
 # 2^-17 relative rounding of inputs / weights / hidden activations).  Tolerance on composited features: 3e-5 (fp32),
 # 2e-4 (tc) absolute on O(1) values; depth and weights only depend on the decoder through sigma.

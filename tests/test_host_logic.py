@@ -64,7 +64,7 @@ def test_synthesis_contract(G):
 
 
 def test_layout_and_chaining_switches_do_not_change_values(G):
-    """The B200 host-side choices -- NHWC activations, epilogues that pre-modulate the next layer, activation scaling
+    """The GPU build's host-side choices -- NHWC activations, epilogues that pre-modulate the next layer, activation scaling
     instead of weight modulation -- are re-orderings of the reference arithmetic (inversion/networks.py:97-129)."""
     from ide3d_b200.training import networks as nw
     z = torch.randn(2, G.z_dim, generator=torch.Generator().manual_seed(3))
