@@ -90,6 +90,13 @@ class RaymarchParams(C.Structure):
                 ('out_feat', C.c_void_p), ('out_depth', C.c_void_p), ('out_weights', C.c_void_p), ('precision', C.c_int)]
 
 
+class RasterParams(C.Structure):
+    _fields_ = [('vertices', C.c_void_p), ('triangles', C.c_void_p), ('normals', C.c_void_p), ('cam2world', C.c_void_p),
+                ('num_vertices', C.c_int64), ('num_triangles', C.c_int64), ('num_frames', C.c_int), ('width', C.c_int), ('height', C.c_int),
+                ('yfov_deg', C.c_float), ('znear', C.c_float), ('base', C.c_float), ('ambient', C.c_float), ('diffuse', C.c_float),
+                ('background', C.c_int), ('rgb', C.c_void_p), ('ids', C.c_void_p), ('scratch', C.c_void_p), ('scratch_bytes', C.c_int64)]
+
+
 _lib = None
 
 
@@ -158,9 +165,13 @@ def get_lib():
     lib.ide3d_mc_classify.argtypes = [vp, i32, i32, i32, f32, vp, vp, vp]
     lib.ide3d_mc_emit.argtypes = [vp, i32, i32, i32, f32, vp, vp, vp, vp, vp, vp, vp]
     lib.ide3d_style_plan.argtypes = [vp, i32, i32, i32, C.POINTER(StyleLayer), i32, vp, vp, vp]
+    lib.ide3d_mesh_normals.argtypes = [vp, vp, i64, vp, vp, vp, vp]
+    lib.ide3d_raster_scratch_bytes.argtypes = [i32, i32, i32, i64, i64]
+    lib.ide3d_raster_scratch_bytes.restype = C.c_int64
+    lib.ide3d_raster.argtypes = [C.POINTER(RasterParams), vp]
     for name in ('bias_act', 'upfirdn2d', 'filtered_lrelu', 'filtered_lrelu_act', 'raymarch_fwd', 'raymarch_bwd', 'sample_voxel',
                  'sigma_grid', 'planes_to_nhwc', 'initial_rays', 'transform_points', 'sample_triplane', 'integrate',
-                 'sample_pdf', 'style_plan', 'mc_classify', 'mc_emit', 'abi_version'):
+                 'sample_pdf', 'style_plan', 'mc_classify', 'mc_emit', 'mesh_normals', 'raster', 'abi_version'):
         getattr(lib, 'ide3d_' + name).restype = C.c_int
     if lib.ide3d_abi_version() != 1:
         raise RuntimeError('ide3d_b200: ABI version mismatch between _lib.py and libide3d_b200.so')
@@ -174,7 +185,8 @@ def exported_symbols():
             'ide3d_upfirdn2d', 'ide3d_upfirdn2d_add', 'ide3d_upfirdn2d_epilogue',
             'ide3d_filtered_lrelu', 'ide3d_filtered_lrelu_act', 'ide3d_raymarch_fwd', 'ide3d_raymarch_bwd', 'ide3d_sample_voxel',
             'ide3d_sigma_grid', 'ide3d_planes_to_nhwc', 'ide3d_initial_rays', 'ide3d_transform_points',
-            'ide3d_sample_triplane', 'ide3d_integrate', 'ide3d_sample_pdf', 'ide3d_mask2color', 'ide3d_style_plan', 'ide3d_mc_classify', 'ide3d_mc_emit']
+            'ide3d_sample_triplane', 'ide3d_integrate', 'ide3d_sample_pdf', 'ide3d_mask2color', 'ide3d_style_plan', 'ide3d_mc_classify', 'ide3d_mc_emit',
+            'ide3d_mesh_normals', 'ide3d_raster_scratch_bytes', 'ide3d_raster']
 
 
 def check(rc, allow_unsupported=False):

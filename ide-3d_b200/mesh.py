@@ -13,9 +13,13 @@ choices on ambiguous faces are not recoverable here, so parity with it is unpinn
 Euler characteristic, vertices on the iso-level, area / volume of analytic shapes) and the CUDA kernels against the numpy oracle bit for bit.
 
     vertices, triangles = marching_cubes(volume, threshold)      # volume: CUDA tensor [nx, ny, nz] (any float dtype)
+
+The rest of render_mesh.py (:36-67, a shaded turntable drawn with pyrender) is `render_turntable`: smooth normals (`vertex_normals`) and
+the frames (`rasterize`, csrc/raster.cu) on the device, the camera path of the reference (`turntable_poses`).
 """
 
 import ctypes as C
+import math
 
 import numpy as np
 import torch
@@ -140,3 +144,103 @@ def mesh_from_sigma_grid(sigma, size=None, sigma_threshold=10.0):
     size = sigma.shape[0] if size is None else size
     vertices, triangles = marching_cubes(torch.clamp_min(sigma, 0), sigma_threshold)
     return vertices / float(size), triangles
+
+
+# ---------------------------------------------------------------------------------------------------------------- rendering
+# render_mesh.py:36-67 draws the mesh with pyrender (OpenGL offscreen, which needs a GL context).  Here: csrc/raster.cu, a visibility
+# buffer resolved by 64-bit atomics, one call per batch of frames.  The camera path and projection are the reference's; the shading is
+# this project's stated choice (DESIGN.md §3): grey, two-sided Lambert headlight plus ambient, no anti-aliasing, no culling.
+MATERIAL = dict(base=0.85, ambient=0.25, diffuse=0.75, background=255)
+
+
+def _check_mesh(vertices, triangles):
+    L.require_cuda(vertices, triangles)
+    if vertices.ndim != 2 or vertices.shape[1] != 3 or triangles.ndim != 2 or triangles.shape[1] != 3:
+        raise ValueError('mesh: vertices must be [V, 3] and triangles [T, 3]')
+    if vertices.shape[0] >= 2 ** 31 or triangles.shape[0] >= 2 ** 31:
+        raise ValueError('mesh: at most 2^31 - 1 vertices and triangles')
+    v = vertices.detach().to(torch.float32).contiguous()
+    t = triangles.detach().to(device=v.device, dtype=torch.int32).contiguous()
+    if t.numel() and (int(t.min()) < 0 or int(t.max()) >= v.shape[0]):
+        raise ValueError('mesh: triangle index out of range')
+    return v, t
+
+
+@torch.no_grad()
+def vertex_normals(vertices, triangles):
+    """Smooth vertex normals (trimesh's, used by pyrender with smooth=True): per vertex the sum of its faces' cross products
+    (area-weighted), normalised; (0, 0, 0) where the sum vanishes.  The vertex -> face adjacency is sorted here once, so the
+    kernel sums in a fixed order and the result is the same on every run.  -> [V, 3] float32 on the vertices' device."""
+    v, t = _check_mesh(vertices, triangles)
+    V = v.shape[0]
+    normals = torch.zeros(V, 3, dtype=torch.float32, device=v.device)
+    if V == 0 or t.shape[0] == 0:
+        return normals
+    flat = t.reshape(-1).long()
+    faces = (torch.sort(flat, stable=True)[1] // 3).to(torch.int32)               # stable: ascending face index per vertex
+    offsets = torch.zeros(V + 1, dtype=torch.int32, device=v.device)
+    offsets[1:] = torch.cumsum(torch.bincount(flat, minlength=V), 0)
+    L.check(L.get_lib().ide3d_mesh_normals(L.ptr(v), L.ptr(t), V, L.ptr(offsets), L.ptr(faces), L.ptr(normals), L.stream_ptr(v.device)))
+    return normals
+
+
+def turntable_poses(w_frames=240, radius=2.7):
+    """render_mesh.py:44-55: cam2world [F, 4, 4] float32 (CPU) of the turntable that circles the unit-cube mesh, looking at its
+    centre (0.5, 0.5, 0.5).  Computed as the reference does, per frame with sample_camera_positions / create_cam2world_matrix."""
+    from .training.volumetric_rendering import create_cam2world_matrix, sample_camera_positions
+    poses = []
+    for i in range(w_frames):
+        yaw = math.pi * (0.5 + 0.15 * math.cos(2 * math.pi * i / w_frames))
+        pitch = math.pi * (0.5 - 0.05 * math.sin(2 * math.pi * i / w_frames))
+        p, _, _ = sample_camera_positions(None, n=1, r=radius, horizontal_mean=yaw, vertical_mean=pitch, mode=None)
+        P = create_cam2world_matrix(-p, p, device=None).reshape(-1, 4, 4)[0].clone()
+        P[:3, 3] += 0.5
+        poses.append(P)
+    return torch.stack(poses) if poses else torch.zeros(0, 4, 4)
+
+
+@torch.no_grad()
+def rasterize(vertices, triangles, cam2world, resolution=512, yfov=18.0, znear=0.05, normals=None, return_ids=False, **material):
+    """Shaded frames of one mesh, one per camera: pyrender's PerspectiveCamera(yfov) on an OffscreenRenderer (OpenGL axes, aspect
+    W / H, row 0 at the top) with a headlight.  vertices [V,3], triangles [T,3] on a CUDA device; cam2world [F,4,4] or [F,16], rigid;
+    resolution: int or (W, H); material: base, ambient, diffuse (floats) and background (0..255), defaults MATERIAL.
+    -> rgb uint8 [F,H,W,3] (and ids int32 [F,H,W], the visible triangle or -1, with return_ids)."""
+    unknown = set(material) - set(MATERIAL)
+    if unknown:
+        raise TypeError(f'rasterize: unknown material keys {sorted(unknown)}')
+    mat = dict(MATERIAL, **material)
+    v, t = _check_mesh(vertices, triangles)
+    dev = v.device
+    W, H = (resolution, resolution) if isinstance(resolution, int) else (int(resolution[0]), int(resolution[1]))
+    c2w = torch.as_tensor(cam2world).detach().to(device=dev, dtype=torch.float32).reshape(-1, 16).contiguous()
+    F = c2w.shape[0]
+    n = vertex_normals(v, t) if normals is None else normals.detach().to(device=dev, dtype=torch.float32).contiguous()
+    if n.shape != v.shape:
+        raise ValueError('rasterize: normals must be [V, 3] like the vertices')
+    rgb = torch.empty(F, H, W, 3, dtype=torch.uint8, device=dev)
+    ids = torch.empty(F, H, W, dtype=torch.int32, device=dev) if return_ids else None
+    lib = L.get_lib()
+    need = int(lib.ide3d_raster_scratch_bytes(F, W, H, v.shape[0], t.shape[0]))
+    if need < 0:
+        raise ValueError(f'rasterize: bad sizes (frames {F}, resolution {W} x {H})')
+    scratch = torch.empty(max(need, 1), dtype=torch.uint8, device=dev)          # caching-allocator blocks are 512-byte aligned
+    p = L.RasterParams(L.ptr(v), L.ptr(t), L.ptr(n), L.ptr(c2w), v.shape[0], t.shape[0], F, W, H, float(yfov), float(znear),
+                       float(mat['base']), float(mat['ambient']), float(mat['diffuse']), int(mat['background']),
+                       L.ptr(rgb), L.ptr(ids), L.ptr(scratch), scratch.numel())
+    L.check(lib.ide3d_raster(C.byref(p), L.stream_ptr(dev)))
+    return (rgb, ids) if return_ids else rgb
+
+
+@torch.no_grad()
+def render_turntable(sigma, size=None, sigma_threshold=10.0, w_frames=240, resolution=512, batch=8, **material):
+    """render_mesh.render on the device: marching cubes of the clamped density grid (mesh_from_sigma_grid), the normals once, then
+    the turntable frames rasterised `batch` at a time.  sigma: [n,n,n] (or flat n^3) CUDA tensor.  -> uint8 [F, H, W, 3] on its device."""
+    vertices, triangles = mesh_from_sigma_grid(sigma, size=size, sigma_threshold=sigma_threshold)
+    normals = vertex_normals(vertices, triangles)
+    poses = turntable_poses(w_frames)
+    frames = [rasterize(vertices, triangles, poses[k:k + batch], resolution=resolution, normals=normals, **material)
+              for k in range(0, w_frames, batch)]
+    if not frames:
+        W, H = (resolution, resolution) if isinstance(resolution, int) else resolution
+        return torch.zeros(0, H, W, 3, dtype=torch.uint8, device=sigma.device)
+    return torch.cat(frames)

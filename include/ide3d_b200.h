@@ -22,6 +22,8 @@
  *   ide3d_raymarch_fwd        the per-frame chain the generator class runs: rays -> jitter -> world
  *                             transform -> 2x tri-plane gather -> decoder MLP -> compositing, fused.
  *   ide3d_planes_to_nhwc      layout helper for the two kernels above (no reference counterpart).
+ *   ide3d_mesh_normals        render_mesh.py:36-42  smooth vertex normals (trimesh / pyrender smooth=True)
+ *   ide3d_raster              render_mesh.py:44-61  shaded frames of the mesh (pyrender OffscreenRenderer)
  *
  * Conventions
  *   - plain C: raw device pointers, sizes, strides (in ELEMENTS), a cudaStream_t passed as void*.
@@ -314,6 +316,49 @@ int ide3d_mc_classify(const float* volume, int nx, int ny, int nz, float thresho
                       ide3d_stream_t stream);
 int ide3d_mc_emit(const float* volume, int nx, int ny, int nz, float threshold, const signed char* tri_table, const int* edge_corner,
                   const unsigned char* counts, const int64_t* offsets, int64_t* edge_ids, float* verts, ide3d_stream_t stream);
+
+/* Mesh rendering (render_mesh.py:36-67 draws the marching-cubes mesh with pyrender / OpenGL offscreen; this is a visibility-buffer
+ * rasteriser instead, no graphics context).
+ *
+ * ide3d_mesh_normals: smooth vertex normals.  normals[v] = normalise(sum over the faces f of v, in adjacency order, of
+ * cross(p1 - p0, p2 - p0)) -- the area-weighted face normals -- or (0, 0, 0) when the sum is zero.  vertices [V,3] fp32, triangles
+ * [T,3] int32; the adjacency is CSR: the faces of vertex v are adj_faces[adj_offsets[v] .. adj_offsets[v+1]) (int32, ascending face
+ * index is what ide3d_b200/mesh.py builds).  No atomics: the result is deterministic.
+ *
+ * ide3d_raster: F frames of one mesh in one call.  Camera: cam2world [F,16] row-major, RIGID (rotation + translation); OpenGL
+ * convention (looks down -z, +y up), vertical field of view yfov_deg, aspect width / height, near plane znear, no far plane.
+ * Image row 0 is the top, pixel centres at half-integers, one sample per pixel (no anti-aliasing), no culling.
+ *   - screen positions are snapped to 1/256 pixel (round half to even); coverage by exact int64 edge functions with the top-left
+ *     fill rule, so triangles sharing an edge cover each pixel centre on it exactly once;
+ *   - a triangle is dropped when a vertex has view depth w < znear, or lies more than 16384 pixels outside the viewport (guard band);
+ *   - visibility: per pixel the minimum of (bits of the fp32 view depth) << 32 | triangle index, i.e. the nearest surface, ties to the
+ *     lower triangle index, independent of launch order;
+ *   - shading, grey, two-sided headlight: c = base * clamp(ambient + diffuse * |n . l|, 0, 1), n the perspective-correct interpolated
+ *     vertex normal (normalised), l the camera's view direction; stored as round(255 c) in all three channels.  background: 0..255.
+ * Outputs: rgb uint8 [F,H,W,3]; ids int32 [F,H,W] (visible triangle, -1 for background) or NULL.
+ * scratch: caller-owned device memory, 256-byte aligned, at least ide3d_raster_scratch_bytes(F, W, H, V, T) bytes (a key buffer of
+ * 8 bytes per pixel, 16 bytes per frame and vertex, 8 bytes per frame and triangle); contents on entry do not matter.
+ * Limits: 1 <= width, height <= 16384; V, T < 2^31; F * T < 2^32. */
+typedef struct ide3d_raster_params {
+    const float* vertices;      /* [V,3] */
+    const int32_t* triangles;   /* [T,3] */
+    const float* normals;       /* [V,3] (ide3d_mesh_normals) */
+    const float* cam2world;     /* [F,16] */
+    int64_t num_vertices, num_triangles;
+    int num_frames, width, height;
+    float yfov_deg, znear;
+    float base, ambient, diffuse;
+    int background;
+    uint8_t* rgb;               /* [F,H,W,3] */
+    int32_t* ids;               /* [F,H,W] or NULL */
+    void* scratch;
+    int64_t scratch_bytes;
+} ide3d_raster_params;
+int ide3d_mesh_normals(const float* vertices, const int32_t* triangles, int64_t num_vertices, const int32_t* adj_offsets,
+                       const int32_t* adj_faces, float* normals, ide3d_stream_t stream);
+/* bytes of scratch ide3d_raster needs; -1 for negative arguments */
+int64_t ide3d_raster_scratch_bytes(int num_frames, int width, int height, int64_t num_vertices, int64_t num_triangles);
+int ide3d_raster(const ide3d_raster_params* p, ide3d_stream_t stream);
 
 /* Style vectors and demodulation coefficients of every modulated convolution of one synthesis call, two launches
  * (replaces per layer: FullyConnectedLayer.forward of the affine, inversion/networks.py:136-165 / :476, and the dcoefs
