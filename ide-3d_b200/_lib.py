@@ -97,6 +97,18 @@ class RasterParams(C.Structure):
                 ('background', C.c_int), ('rgb', C.c_void_p), ('ids', C.c_void_p), ('scratch', C.c_void_p), ('scratch_bytes', C.c_int64)]
 
 
+FRAMES_IMAGE_SEG, FRAMES_IMAGE_DEPTH = 1, 2
+FRAMES_PARTIALS = 64                                   # IDE3D_FRAMES_PARTIALS
+
+
+class FramesParams(C.Structure):
+    _fields_ = [('image', C.c_void_p), ('n', C.c_int), ('height', C.c_int), ('width', C.c_int),
+                ('image_stride_n', C.c_int64), ('image_stride_c', C.c_int64), ('image_stride_h', C.c_int64), ('image_stride_w', C.c_int64),
+                ('seg', C.c_void_p), ('seg_c', C.c_int), ('seg_h', C.c_int), ('seg_w', C.c_int),
+                ('seg_stride_n', C.c_int64), ('seg_stride_c', C.c_int64), ('seg_stride_h', C.c_int64), ('seg_stride_w', C.c_int64),
+                ('lut', C.c_void_p), ('mode', C.c_int), ('out', C.c_void_p), ('scratch', C.c_void_p)]
+
+
 _lib = None
 
 
@@ -169,9 +181,10 @@ def get_lib():
     lib.ide3d_raster_scratch_bytes.argtypes = [i32, i32, i32, i64, i64]
     lib.ide3d_raster_scratch_bytes.restype = C.c_int64
     lib.ide3d_raster.argtypes = [C.POINTER(RasterParams), vp]
+    lib.ide3d_video_frames.argtypes = [C.POINTER(FramesParams), vp]
     for name in ('bias_act', 'upfirdn2d', 'filtered_lrelu', 'filtered_lrelu_act', 'raymarch_fwd', 'raymarch_bwd', 'sample_voxel',
                  'sigma_grid', 'planes_to_nhwc', 'initial_rays', 'transform_points', 'sample_triplane', 'integrate',
-                 'sample_pdf', 'style_plan', 'mc_classify', 'mc_emit', 'mesh_normals', 'raster', 'abi_version'):
+                 'sample_pdf', 'style_plan', 'mc_classify', 'mc_emit', 'mesh_normals', 'raster', 'video_frames', 'abi_version'):
         getattr(lib, 'ide3d_' + name).restype = C.c_int
     if lib.ide3d_abi_version() != 1:
         raise RuntimeError('ide3d_b200: ABI version mismatch between _lib.py and libide3d_b200.so')
@@ -186,7 +199,7 @@ def exported_symbols():
             'ide3d_filtered_lrelu', 'ide3d_filtered_lrelu_act', 'ide3d_raymarch_fwd', 'ide3d_raymarch_bwd', 'ide3d_sample_voxel',
             'ide3d_sigma_grid', 'ide3d_planes_to_nhwc', 'ide3d_initial_rays', 'ide3d_transform_points',
             'ide3d_sample_triplane', 'ide3d_integrate', 'ide3d_sample_pdf', 'ide3d_mask2color', 'ide3d_style_plan', 'ide3d_mc_classify', 'ide3d_mc_emit',
-            'ide3d_mesh_normals', 'ide3d_raster_scratch_bytes', 'ide3d_raster']
+            'ide3d_mesh_normals', 'ide3d_raster_scratch_bytes', 'ide3d_raster', 'ide3d_video_frames']
 
 
 def check(rc, allow_unsupported=False):

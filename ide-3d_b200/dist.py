@@ -11,6 +11,8 @@ import os
 import torch
 import torch.distributed as dist
 
+from . import video
+
 
 def init_from_env(backend=None):
     """Initialise torch.distributed from torchrun's env (RANK / WORLD_SIZE / LOCAL_RANK / MASTER_*).
@@ -147,10 +149,12 @@ def _shared_frame_buffer(shape, rank, world, tag):
 
 
 @torch.no_grad()
-def stream_frames_sharded(G, ws, c, rank, world, batch=8, out=None, transport='auto', **synthesis_kwargs):
+def stream_frames_sharded(G, ws, c, rank, world, batch=8, out=None, transport='auto', image_mode='image', **synthesis_kwargs):
     """The frame loop of gen_videos.py:127-139 as a pipeline: frames i = rank, rank+world, ... are rendered in batches and
     copied to page-locked HOST memory on a side stream while the next batch renders.  ws [F, num_ws, w_dim], c [F, 25] on
-    the host (pinned for asynchronous uploads).  Returns uint8 [F, 3, H, W] on the host on rank 0, None elsewhere.
+    the host (pinned for asynchronous uploads).  Returns uint8 [F, 3, H, k*W] on the host on rank 0, None elsewhere: image_mode
+    (gen_videos.py:130-135) 'image' (k = 1), 'image_seg' (image | colourised semantic mask, k = 2) or 'image_depth' (the negated image
+    min/max-normalised per frame, k = 1); the last two are composed by video.compose_frames from the render-resolution logits.
     F must be a multiple of world * batch.  The returned tensor is a cached buffer (pinned, or the shared one): it is valid until the
     next call with the same frame count -- consume or copy it before calling again (pass `out=` to get a private copy).
 
@@ -161,21 +165,24 @@ def stream_frames_sharded(G, ws, c, rank, world, batch=8, out=None, transport='a
               round-1 path; also what the gloo CPU tests exercise, and the only choice across boxes)."""
     F = ws.shape[0]
     assert F % (world * batch) == 0, 'stream_frames_sharded: F must be a multiple of world * batch'
+    if image_mode not in video.FRAME_WIDTH:
+        raise ValueError(f'stream_frames_sharded: image_mode must be one of {sorted(video.FRAME_WIDTH)}, got {image_mode!r}')
+    width = video.FRAME_WIDTH[image_mode] * G.img_resolution
     dev = next(G.parameters()).device
     cuda = dev.type == 'cuda'
     if transport == 'auto':
         transport = 'shm' if (cuda and world > 1 and os.path.isdir('/dev/shm')) else 'nccl'
         if transport == 'shm':
             # the shared buffer must fit /dev/shm (containers often cap it): rank 0 looks, everybody follows its decision
-            shape_key = (F, G.img_channels, G.img_resolution, G.img_resolution)
-            need = F * G.img_channels * G.img_resolution * G.img_resolution
+            shape_key = (F, G.img_channels, G.img_resolution, width)
+            need = F * G.img_channels * G.img_resolution * width
             ok = torch.zeros(1, dtype=torch.int32, device=dev)
             if rank == 0 and ((shape_key, 'frames') in _shared or _shm_free_bytes() > need + (64 << 20)):
                 ok += 1
             dist.broadcast(ok, src=0)
             if int(ok.item()) == 0:
                 transport = 'nccl'
-    shape = (F, G.img_channels, G.img_resolution, G.img_resolution)
+    shape = (F, G.img_channels, G.img_resolution, width)
     host = None
     if world > 1 and transport == 'shm':
         host = _shared_frame_buffer(shape, rank, world, 'frames')
@@ -189,10 +196,17 @@ def stream_frames_sharded(G, ws, c, rank, world, batch=8, out=None, transport='a
         else:
             sel = torch.arange(rank + world * b0, rank + world * (b0 + batch), world)
             w_b, c_b = ws[sel], c[sel]
-        img = G.synthesis(w_b.to(dev, non_blocking=True), c=c_b.to(dev, non_blocking=True), **synthesis_kwargs)
-        if isinstance(img, (tuple, list)):
-            img = img[0]
-        img = (img * 127.5 + 128).clamp(0, 255).to(torch.uint8).contiguous()
+        if image_mode == 'image_seg':
+            img, seg_raw = G.synthesis(w_b.to(dev, non_blocking=True), c=c_b.to(dev, non_blocking=True), return_seg='raw', **synthesis_kwargs)
+            img = video.compose_frames(img, seg_raw, image_mode)
+        else:
+            img = G.synthesis(w_b.to(dev, non_blocking=True), c=c_b.to(dev, non_blocking=True), **synthesis_kwargs)
+            if isinstance(img, (tuple, list)):
+                img = img[0]
+            if image_mode == 'image_depth':
+                img = video.compose_frames(img, None, image_mode)
+            else:
+                img = (img * 127.5 + 128).clamp(0, 255).to(torch.uint8).contiguous()
         if world > 1 and transport == 'shm':
             # my frames k of this batch are global frames rank + world * (b0 + k): one asynchronous copy per frame into the shared buffer
             if cuda:

@@ -7,6 +7,8 @@ Contract reconstructed from the call sites (SURVEY.md §8b):
     G.mapping(z, c, truncation_psi=1, truncation_cutoff=None) -> ws [N, 18, w_dim];  G.mapping.w_avg
     G.synthesis(ws, c=None, render_params=None, noise_mode='const', force_fp32=False, return_seg=False,
                 return_raw=False) -> img [N,3,512,512] | (img, seg [N,19,512,512]) | (img, img_raw)
+        return_seg='raw' (extension): (img, seg_raw [N,19,R,R]), the render-resolution logits as a strided view of the
+        ray-march output, not upsampled
     G.synthesis.voxel_block_resolutions / vb{res}(x, img, ws, condition_img=seg) -> (x, img, seg)
     G.synthesis.block_resolutions / b{res};  .num_ws, .w_dim, .render_size
     G.synthesis.renderer.sample_voxel(img_v, seg_v, points [N,P,3]) -> [N,P,52]       (extract_shapes.py:146)
@@ -136,6 +138,12 @@ class TriPlaneRenderer(torch.nn.Module):
 
 
 # ================================================================================================ synthesis
+def upsample_seg(seg_raw, size):
+    """Render-resolution semantic logits [N, 19, R, R] -> image resolution: bilinear, align_corners=False.  The rule of
+    return_seg=True / return_dict; ide3d_video_frames (csrc/frames.cu) evaluates the same rule per pixel instead."""
+    return torch.nn.functional.interpolate(seg_raw, size=size, mode='bilinear', align_corners=False)
+
+
 @persistence.persistent_class
 class SynthesisNetwork(torch.nn.Module):
     def __init__(self, w_dim, img_resolution=512, img_channels=3, plane_resolution=256, plane_channels=96,
@@ -260,10 +268,11 @@ class SynthesisNetwork(torch.nn.Module):
         if return_dict:
             return dict(image=img, image_raw=feat_img[:, :self.img_channels],
                         image_depth=depth.permute(0, 2, 1).reshape(n, 1, R, R),
-                        image_seg=torch.nn.functional.interpolate(seg_raw, size=out_size, mode='bilinear', align_corners=False))
+                        image_seg=upsample_seg(seg_raw, out_size))
+        if return_seg == 'raw':
+            return img, seg_raw
         if return_seg:
-            seg = torch.nn.functional.interpolate(seg_raw, size=out_size, mode='bilinear', align_corners=False)
-            return img, seg
+            return img, upsample_seg(seg_raw, out_size)
         if return_raw:
             return img, feat_img[:, :self.img_channels]
         return img

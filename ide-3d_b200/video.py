@@ -8,10 +8,13 @@ ranks, with the host download overlapping the next batch.  Video encoding (image
 result is the uint8 frame grid `layout_grid` (gen_videos.py:24-38) would hand to the writer.
 """
 
+import ctypes as C
 import math
 
 import numpy as np
 import torch
+
+from . import _lib as L
 
 INTRINSICS = [4.2647, 0, 0.5, 0, 4.2647, 0.5, 0, 0, 1]           # gen_videos.py:85
 
@@ -75,12 +78,54 @@ def layout_frames(frames, F, grid_h, grid_w):
     return g.reshape(F, grid_h * ih, grid_w * iw, ch)
 
 
+FRAME_WIDTH = {'image': 1, 'image_seg': 2, 'image_depth': 1}      # cell width in image widths, per image_mode (gen_videos.py:130-135)
+_FRAME_MODES = {'image_seg': L.FRAMES_IMAGE_SEG, 'image_depth': L.FRAMES_IMAGE_DEPTH}
+
+
+def compose_frames(img, seg_raw, image_mode):
+    """The uint8 cells gen_interp_video writes in the image_seg / image_depth modes (gen_videos.py:129-139, then layout_grid's
+    conversion :29-30), in one fused pass (ide3d_video_frames).  img [N, 3, H, W] float32, any strides; seg_raw [N, C, h, w] float32,
+    any strides -- the render-resolution logits of G.synthesis(..., return_seg='raw'), upsampled inside the kernel by the rule of
+    training.triplane.upsample_seg -- for image_seg, ignored for image_depth.  Returns uint8 [N, 3, H, k*W] (k = FRAME_WIDTH[image_mode]).
+    image_depth normalises every frame by its own min / max, as the reference's batch-1 calls do.  CUDA tensors only."""
+    if image_mode not in _FRAME_MODES:
+        raise ValueError(f"compose_frames: image_mode must be one of {sorted(_FRAME_MODES)}, got {image_mode!r} ('image' frames are "
+                         f"the plain uint8 conversion of the image)")
+    seg = seg_raw if image_mode == 'image_seg' else None
+    L.require_cuda(img, seg)
+    L.forbid_grad('video.compose_frames', img, seg)
+    for name, t in (('img', img), ('seg_raw', seg)):
+        if t is not None and (t.dtype != torch.float32 or t.ndim != 4):
+            raise RuntimeError(f'ide3d_b200.video.compose_frames: {name} must be float32 [N, C, H, W], got {t.dtype} {tuple(t.shape)}')
+    n, ch, h, w = img.shape
+    if ch != 3:
+        raise RuntimeError(f'ide3d_b200.video.compose_frames: img must have 3 channels, got {ch}')
+    out = torch.empty([n, 3, h, FRAME_WIDTH[image_mode] * w], dtype=torch.uint8, device=img.device)
+    p = L.FramesParams()
+    p.image, p.n, p.height, p.width = img.data_ptr(), n, h, w
+    p.image_stride_n, p.image_stride_c, p.image_stride_h, p.image_stride_w = img.stride()
+    p.mode, p.out = _FRAME_MODES[image_mode], out.data_ptr()
+    if seg is not None:
+        if seg.shape[0] != n:
+            raise RuntimeError(f'ide3d_b200.video.compose_frames: {n} images but {seg.shape[0]} logit maps')
+        from .dnnlib.seg_tools import _lut_for
+        p.seg, (p.seg_c, p.seg_h, p.seg_w) = seg.data_ptr(), seg.shape[1:]
+        p.seg_stride_n, p.seg_stride_c, p.seg_stride_h, p.seg_stride_w = seg.stride()
+        p.lut = _lut_for(seg.device, seg.shape[1]).data_ptr()
+    else:
+        scratch = torch.empty([max(n, 1) * L.FRAMES_PARTIALS * 2], dtype=torch.float32, device=img.device)
+        p.scratch = scratch.data_ptr()
+    L.check(L.get_lib().ide3d_video_frames(C.byref(p), L.stream_ptr(img.device)))
+    return out
+
+
 @torch.no_grad()
-def render_interp_video(G, seeds, rank=0, world=1, batch=8, out=None, synthesis_kwargs=None, **kwargs):
-    """All frames of gen_interp_video (image_mode='image') as uint8 grids [F, grid_h*H, grid_w*W, 3] on the host of rank 0
-    (None on the other ranks).  kwargs: the arguments of `interp_video_inputs`; synthesis_kwargs: extra arguments of
-    G.synthesis (default noise_mode='const' like gen_videos.py:129; the depth jitter is drawn per batch as in the reference).
-    F * grid cells must be a multiple of world * batch (pad the seed list or pick the batch accordingly)."""
+def render_interp_video(G, seeds, rank=0, world=1, batch=8, out=None, synthesis_kwargs=None, image_mode='image', **kwargs):
+    """All frames of gen_interp_video as uint8 grids [F, grid_h*H, grid_w*k*W, 3] on the host of rank 0 (None on the other ranks);
+    image_mode as in gen_videos.py:184 -- 'image' (k = 1), 'image_seg' (the image with its colourised semantic mask on the right,
+    k = 2) or 'image_depth' (the negated image, min/max-normalised per cell, k = 1).  kwargs: the arguments of `interp_video_inputs`;
+    synthesis_kwargs: extra arguments of G.synthesis (default noise_mode='const' like gen_videos.py:129; the depth jitter is drawn per
+    batch as in the reference).  F * grid cells must be a multiple of world * batch (pad the seed list or pick the batch accordingly)."""
     from . import dist as idist
     ws, c, (F, gh, gw) = interp_video_inputs(G, seeds, **kwargs)
     pin = torch.cuda.is_available()
@@ -90,5 +135,5 @@ def render_interp_video(G, seeds, rank=0, world=1, batch=8, out=None, synthesis_
         ws32, c32 = ws32.pin_memory(), c32.pin_memory()
     skw = dict(noise_mode='const')
     skw.update(synthesis_kwargs or {})
-    frames = idist.stream_frames_sharded(G, ws32, c32, rank, world, batch=batch, out=out, **skw)
+    frames = idist.stream_frames_sharded(G, ws32, c32, rank, world, batch=batch, out=out, image_mode=image_mode, **skw)
     return None if frames is None else layout_frames(frames, F, gh, gw)

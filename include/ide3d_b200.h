@@ -17,6 +17,7 @@
  *   ide3d_integrate           training/volumetric_rendering.py:34   fancy_integration
  *   ide3d_sample_pdf          training/volumetric_rendering.py:224  sample_pdf
  *   ide3d_mask2color          dnnlib/seg_tools.py:75                mask2color
+ *   ide3d_video_frames        gen_videos.py:129-139 + layout_grid :24-38  image_seg / image_depth frames, fused
  *   ide3d_sample_voxel        generator.synthesis.renderer.sample_voxel (call site extract_shapes.py:146)
  *   ide3d_sigma_grid          extract_shapes.py:99-150 (create_samples :74-96 + the sample_voxel loop :144-148)
  *   ide3d_raymarch_fwd        the per-frame chain the generator class runs: rays -> jitter -> world
@@ -304,6 +305,33 @@ int ide3d_sample_pdf(const float* bins, const float* weights, const float* u, in
  * `.to(torch.uint8)` that follows in gen_videos.py:24-38 folded in). */
 int ide3d_mask2color(const float* masks, int n, int c, int h, int w, int64_t stride_n, int64_t stride_c, int64_t stride_h,
                      int64_t stride_w, const float* lut, void* out, int out_u8, ide3d_stream_t stream);
+
+/* Video frames of gen_videos.py's image_seg / image_depth modes (gen_videos.py:129-139), in the uint8 form layout_grid hands to the
+ * video writer ((x * 127.5 + 128).clamp(0, 255).to(uint8), :24-38), straight from the synthesis outputs.
+ *   image [n, 3, height, width] fp32, element strides (NCHW or channels-last).
+ *   IDE3D_FRAMES_IMAGE_SEG:   out [n, 3, height, 2 * width]; left half the image, right half the colour of the argmax class (first
+ *       maximum, NaN counts as maximal; lut [seg_c, 3] fp32, the COLOR_MAP rows) of the logits seg [n, seg_c, seg_h, seg_w] (fp32, element
+ *       strides) upsampled per pixel to height x width by interpolate(mode='bilinear', align_corners=False).  The upsampled logits are not
+ *       stored anywhere.
+ *   IDE3D_FRAMES_IMAGE_DEPTH: out [n, 3, height, width]; per frame t = -image, ((t - min t) / (max t - min t)) * 2 - 1.  Two launches;
+ *       scratch holds n * IDE3D_FRAMES_PARTIALS * 2 floats of partial minima / maxima.  A constant frame divides 0 by 0, as the
+ *       reference does.
+ * out is dense.  Every operation is rounded separately, as the reference's torch ops are.  Limits: n <= 65535. */
+#define IDE3D_FRAMES_PARTIALS 64
+enum ide3d_frames_mode { IDE3D_FRAMES_IMAGE_SEG = 1, IDE3D_FRAMES_IMAGE_DEPTH = 2 };
+typedef struct ide3d_frames_params {
+    const float* image;
+    int n, height, width;
+    int64_t image_stride_n, image_stride_c, image_stride_h, image_stride_w;
+    const float* seg;           /* IMAGE_SEG only */
+    int seg_c, seg_h, seg_w;
+    int64_t seg_stride_n, seg_stride_c, seg_stride_h, seg_stride_w;
+    const float* lut;           /* IMAGE_SEG only */
+    int mode;                   /* ide3d_frames_mode */
+    uint8_t* out;
+    float* scratch;             /* IMAGE_DEPTH only */
+} ide3d_frames_params;
+int ide3d_video_frames(const ide3d_frames_params* p, ide3d_stream_t stream);
 
 /* Marching cubes on a density grid (render_mesh.py:30-32 / dnnlib/geometry.py:282-286 call PyMCubes' marching_cubes on the host).
  * volume [nx, ny, nz] fp32 dense (index (x*ny + y)*nz + z); a corner is inside where value >= threshold.  Tables (device memory) come

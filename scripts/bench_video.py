@@ -20,6 +20,7 @@ def main():
     ap.add_argument('--w-frames', type=int, default=120)
     ap.add_argument('--chunk', type=int, default=1024, help='renders per streamed chunk (multiple of world * batch)')
     ap.add_argument('--batch', type=int, default=8)
+    ap.add_argument('--image-mode', default='image', choices=['image', 'image_seg', 'image_depth'], help='gen_videos.py --image_mode')
     args = ap.parse_args()
     from ide3d_b200 import dist as idist, video
     from ide3d_b200.torch_utils import custom_ops
@@ -42,7 +43,7 @@ def main():
     prep_s = time.perf_counter() - t0
     total = ws.shape[0]
     chunk = max(world * args.batch, args.chunk // (world * args.batch) * (world * args.batch))
-    kw = dict(noise_mode='const')
+    kw = dict(noise_mode='const', image_mode=args.image_mode)
     with torch.no_grad():
         idist.stream_frames_sharded(G, ws[:chunk], c[:chunk], rank, world, batch=args.batch, **kw)     # warm-up: cuDNN plans, buffers
         barrier()
@@ -63,7 +64,7 @@ def main():
     if world > 1:
         tdist.all_reduce(t, op=tdist.ReduceOp.MAX)
     if rank == 0:
-        print(json.dumps({'config': f'gen_videos grid=2x2 seeds=0-{args.seeds - 1} w_frames={args.w_frames} (BASELINE configs[2])', 'n_gpus': world,
+        print(json.dumps({'config': f'gen_videos grid=2x2 seeds=0-{args.seeds - 1} w_frames={args.w_frames} (BASELINE configs[2])', 'image_mode': args.image_mode, 'n_gpus': world,
                           'video_frames': F, 'renders': done, 'renders_per_s': done / float(t[0]), 'video_frames_per_s': done / 4 / float(t[0]),
                           'render_wall_s': float(t[0]), 'host_input_prep_s (scipy splines + mapping, per rank, untimed)': prep_s,
                           'chunk_renders': chunk, 'batch': args.batch, 'transport': 'shared page-locked /dev/shm buffer, each rank downloads its own frames' if world > 1 else 'pinned host buffer',
