@@ -68,6 +68,20 @@ inline int sm_count() {
 template <typename T>
 __host__ __device__ inline T ceil_div(T a, T b) { return (a + b - 1) / b; }
 
+// Grid of a persistent kernel: as many CTAs of `threads` threads and `smem` bytes of dynamic shared memory as are resident on
+// the device at once, at most `max_ctas` (the CTAs that have work).  Raises the kernel's dynamic shared-memory limit to `smem`.
+template <typename Kernel>
+inline int persistent_grid(Kernel kern, int threads, size_t smem, long long max_ctas, int& grid) {
+    IDE3D_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int per_sm = 1;
+    IDE3D_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
+    if (per_sm < 1) per_sm = 1;
+    const long long resident = (long long)sm_count() * per_sm;
+    grid = (int)(resident < max_ctas ? resident : max_ctas);
+    if (grid < 1) grid = 1;
+    return IDE3D_OK;
+}
+
 // floor division for possibly negative numerators
 __host__ __device__ inline int floor_div(int a, int b) {
     int q = a / b;

@@ -21,19 +21,7 @@ constexpr int kWarps = 8;
 constexpr int kBlock = kWarps * 32;
 constexpr int kTileX = 4, kTileY = 2;
 
-struct RayArgs {
-    PlaneView tex, seg;
-    ide3d_decoder dec;
-    const float* cam2world;
-    int n, res_w, res_h, steps;
-    float cam_z;          // -1 / tan(fov/2)
-    float ray_start, ray_end, box_scale;
-    int jitter_mode;
-    const float* jitter_u;
-    uint32_t seed_lo, seed_hi;
-    int clamp_mode, last_back, white_back, fill_weight;
-    float max_depth, noise_std;
-    const float* noise;
+struct RayArgs : MarchArgs {
     float *out_feat, *out_depth, *out_weights;
     int tiles_x, tiles_y;
 };
@@ -182,13 +170,8 @@ template <int KIND, bool CL>
 static int launch_raymarch(const RayArgs& a, cudaStream_t st) {
     const size_t smem = (size_t)(DecoderTraits<KIND>::kFloats + kWarps * 32 * kRow) * sizeof(float);
     auto kern = raymarch_kernel<KIND, CL>;
-    IDE3D_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int per_sm = 1;
-    IDE3D_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kBlock, smem));
-    if (per_sm < 1) per_sm = 1;
-    const int num_tiles = a.tiles_x * a.tiles_y * a.n;
-    int grid = sm_count() * per_sm;
-    if (grid > num_tiles) grid = num_tiles;
+    int grid, rc;
+    if ((rc = persistent_grid(kern, kBlock, smem, a.tiles_x * a.tiles_y * a.n, grid)) != IDE3D_OK) return rc;
     kern<<<grid, kBlock, smem, st>>>(a);
     IDE3D_CHECK_LAUNCH("raymarch_kernel");
     return IDE3D_OK;
@@ -200,34 +183,12 @@ int launch_raymarch_tc(const ide3d_raymarch_params* p, bool channels_last, cudaS
 
 using namespace ide3d;
 
-static int check_planes(const ide3d_triplane& t, const char* name) {
-    IDE3D_REQUIRE(t.data != nullptr, "%s: null data", name);
-    IDE3D_REQUIRE(t.n > 0 && t.h > 0 && t.w > 0, "%s: empty tri-plane", name);
-    return IDE3D_OK;
-}
-
-static bool is_channels_last(const ide3d_triplane& t) {
-    return t.stride_c == 1 && (t.stride_w % 4 == 0) && (t.stride_h % 4 == 0) && (t.stride_n % 4 == 0) &&
-           ((reinterpret_cast<uintptr_t>(t.data) & 15) == 0);
-}
-
 extern "C" int ide3d_raymarch_fwd(const ide3d_raymarch_params* p, ide3d_stream_t stream) {
-    IDE3D_REQUIRE(p != nullptr, "raymarch: null params");
     int rc;
-    if ((rc = check_planes(p->tex, "tex")) != IDE3D_OK) return rc;
-    if ((rc = check_planes(p->seg, "seg")) != IDE3D_OK) return rc;
-    IDE3D_REQUIRE(p->tex.h == p->seg.h && p->tex.w == p->seg.w, "raymarch: tex/seg plane sizes differ");
-    IDE3D_REQUIRE(p->n > 0 && p->tex.n == p->n && p->seg.n == p->n, "raymarch: batch mismatch");
-    IDE3D_REQUIRE(p->res_w > 0 && p->res_h > 0 && p->num_steps > 0, "raymarch: empty render");
-    IDE3D_REQUIRE(p->cam2world && p->out_feat && p->out_depth, "raymarch: null camera/output");
-    IDE3D_REQUIRE(p->clamp_mode == IDE3D_CLAMP_SOFTPLUS || p->clamp_mode == IDE3D_CLAMP_RELU,
-                  "Need to choose clamp mode");   // volumetric_rendering.py:51-52
-    IDE3D_REQUIRE(p->jitter_mode >= 0 && p->jitter_mode <= 3, "raymarch: bad jitter mode");
-    IDE3D_REQUIRE((p->jitter_mode != IDE3D_JITTER_TENSOR && p->jitter_mode != IDE3D_JITTER_ZVALS) || p->jitter_u, "raymarch: jitter / depth tensor missing");
-    IDE3D_REQUIRE((long long)p->n * p->res_w * p->res_h * p->num_steps < (1ll << 32),
-                  "raymarch: more than 2^32 samples per call");
+    if ((rc = check_raymarch_params(p)) != IDE3D_OK) return rc;
+    IDE3D_REQUIRE(p->out_feat && p->out_depth, "raymarch: null camera/output");
     IDE3D_REQUIRE(p->precision >= IDE3D_PRECISION_AUTO && p->precision <= IDE3D_PRECISION_TC, "raymarch: bad precision");
-    const bool planes_cl = is_channels_last(p->tex) && is_channels_last(p->seg);
+    const bool planes_cl = planes_channels_last(p->tex) && planes_channels_last(p->seg);
     if (p->precision != IDE3D_PRECISION_FP32) {
         const int rc_tc = launch_raymarch_tc(p, planes_cl, (cudaStream_t)stream);
         if (rc_tc != IDE3D_UNSUPPORTED || p->precision == IDE3D_PRECISION_TC) return rc_tc;
@@ -236,16 +197,7 @@ extern "C" int ide3d_raymarch_fwd(const ide3d_raymarch_params* p, ide3d_stream_t
     if (kind == kDecoderNone) IDE3D_FAIL(IDE3D_UNSUPPORTED, "raymarch: no fused kernel for this decoder shape");
 
     RayArgs a;
-    a.tex = make_view(p->tex); a.seg = make_view(p->seg); a.dec = p->dec;
-    a.cam2world = p->cam2world;
-    a.n = p->n; a.res_w = p->res_w; a.res_h = p->res_h; a.steps = p->num_steps;
-    a.cam_z = (float)(-1.0 / tan((2.0 * 3.14159265358979323846 * (double)p->fov_deg / 360.0) / 2.0));
-    a.ray_start = p->ray_start; a.ray_end = p->ray_end; a.box_scale = p->box_scale;
-    a.jitter_mode = p->jitter_mode; a.jitter_u = p->jitter_u;
-    a.seed_lo = (uint32_t)(p->jitter_seed & 0xffffffffu); a.seed_hi = (uint32_t)(p->jitter_seed >> 32);
-    a.clamp_mode = p->clamp_mode; a.last_back = p->last_back; a.white_back = p->white_back;
-    a.fill_weight = p->fill_weight; a.max_depth = p->max_depth;
-    a.noise_std = p->noise_std; a.noise = (p->noise_std != 0.f) ? p->noise : nullptr;
+    fill_march_args(*p, a);
     a.out_feat = p->out_feat; a.out_depth = p->out_depth; a.out_weights = p->out_weights;
     a.tiles_x = ceil_div(p->res_w, kTileX); a.tiles_y = ceil_div(p->res_h, kTileY);
     const bool cl = planes_cl;

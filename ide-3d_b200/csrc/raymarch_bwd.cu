@@ -26,6 +26,7 @@ constexpr int kBBlock = kBWarps * 32;
 constexpr int kBTileX = 4, kBTileY = 2;
 constexpr int kMaxSteps = 256;                      // per-ray shared-memory arrays
 
+// the fields of MarchArgs (filled by fill_march_args), then the gradients and the tiling
 struct BwdArgs {
     PlaneView tex, seg;
     ide3d_decoder dec;
@@ -403,25 +404,15 @@ using namespace ide3d;
 
 extern "C" int ide3d_raymarch_bwd(const ide3d_raymarch_params* p, const float* grad_feat, const float* grad_depth, float* grad_tex,
                                   float* grad_seg, float* const* grad_params, ide3d_stream_t stream) {
-    IDE3D_REQUIRE(p != nullptr && grad_feat != nullptr, "raymarch_bwd: null argument");
-    IDE3D_REQUIRE(p->n > 0 && p->res_w > 0 && p->res_h > 0 && p->num_steps > 0, "raymarch_bwd: empty render");
-    IDE3D_REQUIRE(p->clamp_mode == IDE3D_CLAMP_SOFTPLUS || p->clamp_mode == IDE3D_CLAMP_RELU, "Need to choose clamp mode");
+    int rc;
+    if ((rc = check_raymarch_params(p)) != IDE3D_OK) return rc;
+    IDE3D_REQUIRE(grad_feat != nullptr, "raymarch_bwd: null argument");
     if (p->num_steps > kMaxSteps) IDE3D_FAIL(IDE3D_UNSUPPORTED, "raymarch_bwd: more than %d samples per ray", kMaxSteps);
     if (classify_decoder(p->dec) != kThreeHead64) IDE3D_FAIL(IDE3D_UNSUPPORTED, "raymarch_bwd: only the three-head decoder has a backward kernel");
-    auto cl = [](const ide3d_triplane& t) {
-        return t.stride_c == 1 && (t.stride_w % 4 == 0) && (t.stride_h % 4 == 0) && (t.stride_n % 4 == 0) && ((reinterpret_cast<uintptr_t>(t.data) & 15) == 0);
-    };
-    if (!cl(p->tex) || !cl(p->seg)) IDE3D_FAIL(IDE3D_UNSUPPORTED, "raymarch_bwd: planes must be channels-last fp32");
+    if (!planes_channels_last(p->tex) || !planes_channels_last(p->seg)) IDE3D_FAIL(IDE3D_UNSUPPORTED, "raymarch_bwd: planes must be channels-last fp32");
     IDE3D_REQUIRE(((reinterpret_cast<uintptr_t>(grad_tex) | reinterpret_cast<uintptr_t>(grad_seg)) & 15) == 0, "raymarch_bwd: plane gradients must be 16-byte aligned");
     BwdArgs a;
-    a.tex = make_view(p->tex); a.seg = make_view(p->seg); a.dec = p->dec; a.cam2world = p->cam2world;
-    a.n = p->n; a.res_w = p->res_w; a.res_h = p->res_h; a.steps = p->num_steps;
-    a.cam_z = (float)(-1.0 / tan((2.0 * 3.14159265358979323846 * (double)p->fov_deg / 360.0) / 2.0));
-    a.ray_start = p->ray_start; a.ray_end = p->ray_end; a.box_scale = p->box_scale;
-    a.jitter_mode = p->jitter_mode; a.jitter_u = p->jitter_u;
-    a.seed_lo = (uint32_t)(p->jitter_seed & 0xffffffffu); a.seed_hi = (uint32_t)(p->jitter_seed >> 32);
-    a.clamp_mode = p->clamp_mode; a.last_back = p->last_back; a.white_back = p->white_back; a.fill_weight = p->fill_weight;
-    a.max_depth = p->max_depth; a.noise_std = p->noise_std; a.noise = (p->noise_std != 0.f) ? p->noise : nullptr;
+    fill_march_args(*p, a);
     a.g_feat = grad_feat; a.g_depth = grad_depth; a.g_tex = grad_tex; a.g_seg = grad_seg;
     const bool params = grad_params != nullptr;
     for (int h = 0; h < 3; ++h)

@@ -1,4 +1,5 @@
-// Device building blocks shared by the fused renderer kernels (raymarch.cu, voxel.cu).
+// Building blocks shared by the fused renderer kernels (raymarch*.cu, voxel*.cu): the ray-march parameter contract (validation,
+// kernel arguments) and the device helpers of the gather, the decoder and the compositing.
 //
 // Data layout in HBM: a tri-plane tensor is [N, 96, H, W] fp32.  The fast path wants it
 // channels-last ([N, H, W, 96]): one texel of one plane = 32 floats = one 128-byte line, fetched by
@@ -32,6 +33,90 @@ inline PlaneView make_view(const ide3d_triplane& t) {
     return v;
 }
 
+// the fast gather's layout: [N, H, W, 96] with every texel on a 16-byte boundary (one LDG.128 per channel quad)
+inline bool planes_channels_last(const ide3d_triplane& t) {
+    return t.stride_c == 1 && (t.stride_w % 4 == 0) && (t.stride_h % 4 == 0) && (t.stride_n % 4 == 0) &&
+           ((reinterpret_cast<uintptr_t>(t.data) & 15) == 0);
+}
+
+// ---------------------------------------------------------------------------------------------
+// the ray-march parameter contract, shared by the forward kernels (raymarch.cu, raymarch_tc.cu) and the backward (raymarch_bwd.cu)
+
+inline int check_planes(const ide3d_triplane& t, const char* name) {
+    IDE3D_REQUIRE(t.data != nullptr, "%s: null data", name);
+    IDE3D_REQUIRE(t.n > 0 && t.h > 0 && t.w > 0, "%s: empty tri-plane", name);
+    return IDE3D_OK;
+}
+
+// Checks of ide3d_raymarch_params that every ray-march entry point needs before it reads the struct.
+inline int check_raymarch_params(const ide3d_raymarch_params* p) {
+    IDE3D_REQUIRE(p != nullptr, "raymarch: null params");
+    int rc;
+    if ((rc = check_planes(p->tex, "tex")) != IDE3D_OK) return rc;
+    if ((rc = check_planes(p->seg, "seg")) != IDE3D_OK) return rc;
+    IDE3D_REQUIRE(p->tex.h == p->seg.h && p->tex.w == p->seg.w, "raymarch: tex/seg plane sizes differ");
+    IDE3D_REQUIRE(p->n > 0 && p->tex.n == p->n && p->seg.n == p->n, "raymarch: batch mismatch");
+    IDE3D_REQUIRE(p->res_w > 0 && p->res_h > 0 && p->num_steps > 0, "raymarch: empty render");
+    IDE3D_REQUIRE(p->cam2world != nullptr, "raymarch: null camera/output");
+    IDE3D_REQUIRE(p->clamp_mode == IDE3D_CLAMP_SOFTPLUS || p->clamp_mode == IDE3D_CLAMP_RELU,
+                  "Need to choose clamp mode");   // volumetric_rendering.py:51-52
+    IDE3D_REQUIRE(p->jitter_mode >= 0 && p->jitter_mode <= 3, "raymarch: bad jitter mode");
+    IDE3D_REQUIRE((p->jitter_mode != IDE3D_JITTER_TENSOR && p->jitter_mode != IDE3D_JITTER_ZVALS) || p->jitter_u, "raymarch: jitter / depth tensor missing");
+    IDE3D_REQUIRE((long long)p->n * p->res_w * p->res_h * p->num_steps < (1ll << 32),
+                  "raymarch: more than 2^32 samples per call");       // the jitter hash indexes samples with 32 bits
+    return IDE3D_OK;
+}
+
+// Kernel arguments every ray-march kernel reads: RayArgs extends it, TcArgs and BwdArgs restate its fields.
+struct MarchArgs {
+    PlaneView tex, seg;
+    ide3d_decoder dec;
+    const float* cam2world;
+    int n, res_w, res_h, steps;
+    float cam_z;          // -1 / tan(fov/2)
+    float ray_start, ray_end, box_scale;
+    int jitter_mode;
+    const float* jitter_u;
+    uint32_t seed_lo, seed_hi;
+    int clamp_mode, last_back, white_back, fill_weight;
+    float max_depth, noise_std;
+    const float* noise;   // null when noise_std == 0
+};
+
+// Args: MarchArgs or a struct with the same fields.  TcArgs and BwdArgs restate them instead of deriving from MarchArgs: as a
+// derived kernel parameter the struct changes the code ptxas emits for those two kernels (3 more registers for raymarch_tc_kernel).
+template <typename Args>
+inline void fill_march_args(const ide3d_raymarch_params& p, Args& a) {
+    a.tex = make_view(p.tex); a.seg = make_view(p.seg); a.dec = p.dec;
+    a.cam2world = p.cam2world;
+    a.n = p.n; a.res_w = p.res_w; a.res_h = p.res_h; a.steps = p.num_steps;
+    a.cam_z = (float)(-1.0 / tan((2.0 * 3.14159265358979323846 * (double)p.fov_deg / 360.0) / 2.0));
+    a.ray_start = p.ray_start; a.ray_end = p.ray_end; a.box_scale = p.box_scale;
+    a.jitter_mode = p.jitter_mode; a.jitter_u = p.jitter_u;
+    a.seed_lo = (uint32_t)(p.jitter_seed & 0xffffffffu); a.seed_hi = (uint32_t)(p.jitter_seed >> 32);
+    a.clamp_mode = p.clamp_mode; a.last_back = p.last_back; a.white_back = p.white_back;
+    a.fill_weight = p.fill_weight; a.max_depth = p.max_depth;
+    a.noise_std = p.noise_std; a.noise = (p.noise_std != 0.f) ? p.noise : nullptr;
+}
+
+// ---------------------------------------------------------------------------------------------
+// point queries (voxel.cu: CUDA cores; voxel_tc.cu: tensor cores, sigma only)
+
+struct VoxelArgs {
+    PlaneView tex, seg;
+    ide3d_decoder dec;
+    const float* points;      // [N, P, 3] or null (grid mode)
+    long long P;              // points per batch item
+    int n;
+    float box_scale;
+    int sigma_only;
+    float* out;
+    // grid mode (extract_shapes.create_samples)
+    int grid_n;
+    float voxel_size, org_x, org_y, org_z, pre_scale;
+    long long first;
+};
+
 // ---------------------------------------------------------------------------------------------
 // scalar helpers
 
@@ -60,6 +145,20 @@ __device__ __forceinline__ float softplus_fast(float x) {
 // density activation: full precision, matters because delta_last = 1e10 amplifies tiny values
 __device__ __forceinline__ float softplus_precise(float x) {
     return fmaxf(x, 0.f) + log1pf(expf(-fabsf(x)));
+}
+
+// coordinates of flat voxel index `idx`, bit-for-bit like extract_shapes.py:74-96 followed by `0.9 *`
+__device__ __forceinline__ void grid_point(const VoxelArgs& a, long long idx, float& x, float& y, float& z) {
+    const float N = (float)a.grid_n;
+    const float fi = (float)idx;                                   // overall_index.float()
+    const float s2 = (float)(idx % a.grid_n);                      // samples[:, 2] = index % N   (integer)
+    const float q1 = __fdiv_rn(fi, N);
+    const float s1 = fmodf(q1, N);                                 // (index.float() / N) % N      (fractional!)
+    const float s0 = fmodf(__fdiv_rn(q1, N), N);                   // ((index.float() / N) / N) % N
+    // column 0 uses voxel_origin[2], column 2 uses voxel_origin[0] (:91-93)
+    x = __fmul_rn(__fadd_rn(__fmul_rn(s0, a.voxel_size), a.org_z), a.pre_scale);
+    y = __fmul_rn(__fadd_rn(__fmul_rn(s1, a.voxel_size), a.org_y), a.pre_scale);
+    z = __fmul_rn(__fadd_rn(__fmul_rn(s2, a.voxel_size), a.org_x), a.pre_scale);
 }
 
 // ---------------------------------------------------------------------------------------------

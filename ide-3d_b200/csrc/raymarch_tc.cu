@@ -288,31 +288,17 @@ int launch_raymarch_tc(const ide3d_raymarch_params* p, bool channels_last, cudaS
     if (!channels_last) IDE3D_FAIL(IDE3D_UNSUPPORTED, "raymarch_tc: planes must be channels-last");
     if (p->tex.stride_h != p->seg.stride_h || p->tex.stride_w != p->seg.stride_w)
         IDE3D_FAIL(IDE3D_UNSUPPORTED, "raymarch_tc: tex and seg planes must share strides");
-    if (((long long)p->tex.h * p->tex.stride_h + (long long)p->tex.w * p->tex.stride_w + 96) * 4 >= (1ll << 31))
-        IDE3D_FAIL(IDE3D_UNSUPPORTED, "raymarch_tc: plane too large for 32-bit byte offsets");
     TcArgs a;
+    fill_march_args(*p, a);
+    if (!plane_fits_32bit(a.tex)) IDE3D_FAIL(IDE3D_UNSUPPORTED, "raymarch_tc: plane too large for 32-bit byte offsets");
     if (!build_program(p->dec, a.prog)) IDE3D_FAIL(IDE3D_UNSUPPORTED, "raymarch_tc: decoder shape not supported");
-    a.tex = make_view(p->tex); a.seg = make_view(p->seg); a.dec = p->dec;
-    a.cam2world = p->cam2world;
-    a.n = p->n; a.res_w = p->res_w; a.res_h = p->res_h; a.steps = p->num_steps;
-    a.cam_z = (float)(-1.0 / tan((2.0 * 3.14159265358979323846 * (double)p->fov_deg / 360.0) / 2.0));
-    a.ray_start = p->ray_start; a.ray_end = p->ray_end; a.box_scale = p->box_scale;
-    a.jitter_mode = p->jitter_mode; a.jitter_u = p->jitter_u;
-    a.seed_lo = (uint32_t)(p->jitter_seed & 0xffffffffu); a.seed_hi = (uint32_t)(p->jitter_seed >> 32);
-    a.clamp_mode = p->clamp_mode; a.last_back = p->last_back; a.white_back = p->white_back;
-    a.fill_weight = p->fill_weight; a.max_depth = p->max_depth;
-    a.noise_std = p->noise_std; a.noise = (p->noise_std != 0.f) ? p->noise : nullptr;
     a.out_feat = p->out_feat; a.out_depth = p->out_depth; a.out_weights = p->out_weights;
     a.units_x = ceil_div(p->res_w, kUnitW); a.units_y = ceil_div(p->res_h, kUnitH);
     a.num_units = a.units_x * a.units_y * a.n;
     a.tiles_per_unit = ceil_div(p->num_steps, kTileDepth);
     const int smem = 2 * a.prog.wpart + kWarpgroups * kStageBytes + (kTcMaxBlocks * 64 + 64) * 4 + 1024;
-    IDE3D_CUDA(cudaFuncSetAttribute(raymarch_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    int per_sm = 1;
-    IDE3D_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, raymarch_tc_kernel, kTcThreads, smem));
-    if (per_sm < 1) per_sm = 1;
-    int grid = sm_count() * per_sm;
-    if (grid * kWarpgroups > a.num_units) grid = ceil_div(a.num_units, kWarpgroups);
+    int grid, rc;
+    if ((rc = persistent_grid(raymarch_tc_kernel, kTcThreads, smem, ceil_div(a.num_units, kWarpgroups), grid)) != IDE3D_OK) return rc;
     raymarch_tc_kernel<<<grid, kTcThreads, smem, st>>>(a);
     IDE3D_CHECK_LAUNCH("raymarch_tc_kernel");
     return IDE3D_OK;

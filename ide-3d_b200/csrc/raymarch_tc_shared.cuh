@@ -28,6 +28,7 @@ struct TcProgram {
     int wpart;                                     // bytes of one weight part (hi or lo), multiple of 1024
 };
 
+// the fields of MarchArgs (filled by fill_march_args), the hidden-block program, outputs and unit tiling
 struct TcArgs {
     PlaneView tex, seg;
     ide3d_decoder dec;
@@ -44,6 +45,11 @@ struct TcArgs {
     float *out_feat, *out_depth, *out_weights;
     int units_x, units_y, num_units, tiles_per_unit;
 };
+
+// gather12 addresses a plane with 32-bit byte offsets
+inline bool plane_fits_32bit(const PlaneView& v) {
+    return ((long long)v.h * v.sh + (long long)v.w * v.sw + 96) * 4 < (1ll << 31);
+}
 
 // log2(1 + 2^t): the hidden softplus in base-2 units (log2e folded into W1 / b1, ln2 into W2 at set-up).  ex2 of the clamped
 // argument cannot overflow; for t >= 24 the sum rounds to 2^t and lg2 returns t itself, max(., t) keeps t beyond the clamp.

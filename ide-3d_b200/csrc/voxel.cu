@@ -10,35 +10,6 @@ namespace ide3d {
 constexpr int kVWarps = 8;
 constexpr int kVBlock = kVWarps * 32;
 
-struct VoxelArgs {
-    PlaneView tex, seg;
-    ide3d_decoder dec;
-    const float* points;      // [N, P, 3] or null (grid mode)
-    long long P;              // points per batch item
-    int n;
-    float box_scale;
-    int sigma_only;
-    float* out;
-    // grid mode (extract_shapes.create_samples)
-    int grid_n;
-    float voxel_size, org_x, org_y, org_z, pre_scale;
-    long long first;
-};
-
-// coordinates of flat voxel index `idx`, bit-for-bit like extract_shapes.py:74-96 followed by `0.9 *`
-__device__ __forceinline__ void grid_point(const VoxelArgs& a, long long idx, float& x, float& y, float& z) {
-    const float N = (float)a.grid_n;
-    const float fi = (float)idx;                                   // overall_index.float()
-    const float s2 = (float)(idx % a.grid_n);                      // samples[:, 2] = index % N   (integer)
-    const float q1 = __fdiv_rn(fi, N);
-    const float s1 = fmodf(q1, N);                                 // (index.float() / N) % N      (fractional!)
-    const float s0 = fmodf(__fdiv_rn(q1, N), N);                   // ((index.float() / N) / N) % N
-    // column 0 uses voxel_origin[2], column 2 uses voxel_origin[0] (:91-93)
-    x = __fmul_rn(__fadd_rn(__fmul_rn(s0, a.voxel_size), a.org_z), a.pre_scale);
-    y = __fmul_rn(__fadd_rn(__fmul_rn(s1, a.voxel_size), a.org_y), a.pre_scale);
-    z = __fmul_rn(__fadd_rn(__fmul_rn(s2, a.voxel_size), a.org_x), a.pre_scale);
-}
-
 template <int KIND, bool kChannelsLast, bool kGrid>
 __global__ void __launch_bounds__(kVBlock, 1) voxel_kernel(const VoxelArgs a) {
     extern __shared__ __align__(16) float smem[];
@@ -98,16 +69,9 @@ template <int KIND, bool CL, bool GRID>
 static int launch_voxel(const VoxelArgs& a, cudaStream_t st) {
     const size_t smem = (size_t)(DecoderTraits<KIND>::kFloats + kVWarps * 32 * kRow) * sizeof(float);
     auto kern = voxel_kernel<KIND, CL, GRID>;
-    IDE3D_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int per_sm = 1;
-    IDE3D_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kVBlock, smem));
-    if (per_sm < 1) per_sm = 1;
-    const long long chunks = ((a.P + 31) >> 5) * a.n;
-    long long grid = (long long)sm_count() * per_sm;
-    const long long need = ceil_div<long long>(chunks, kVWarps);
-    if (grid > need) grid = need;
-    if (grid < 1) grid = 1;
-    kern<<<(unsigned)grid, kVBlock, smem, st>>>(a);
+    int grid, rc;
+    if ((rc = persistent_grid(kern, kVBlock, smem, ceil_div<long long>(((a.P + 31) >> 5) * a.n, kVWarps), grid)) != IDE3D_OK) return rc;
+    kern<<<grid, kVBlock, smem, st>>>(a);
     IDE3D_CHECK_LAUNCH("voxel_kernel");
     return IDE3D_OK;
 }
@@ -148,11 +112,6 @@ __global__ void __launch_bounds__(256) nhwc_kernel(const float* __restrict__ src
     }
 }
 
-static bool view_channels_last(const ide3d_triplane& t) {
-    return t.stride_c == 1 && (t.stride_w % 4 == 0) && (t.stride_h % 4 == 0) && (t.stride_n % 4 == 0) &&
-           ((reinterpret_cast<uintptr_t>(t.data) & 15) == 0);
-}
-
 static int fill_common(VoxelArgs& a, const ide3d_triplane* tex, const ide3d_triplane* seg, const ide3d_decoder* dec,
                        int& kind, bool& cl) {
     IDE3D_REQUIRE(tex && seg && dec, "voxel: null argument");
@@ -162,14 +121,12 @@ static int fill_common(VoxelArgs& a, const ide3d_triplane* tex, const ide3d_trip
     kind = classify_decoder(*dec);
     if (kind == kDecoderNone) IDE3D_FAIL(IDE3D_UNSUPPORTED, "voxel: no fused kernel for this decoder shape");
     a.tex = make_view(*tex); a.seg = make_view(*seg); a.dec = *dec; a.n = tex->n;
-    cl = view_channels_last(*tex) && view_channels_last(*seg);
+    cl = planes_channels_last(*tex) && planes_channels_last(*seg);
     return IDE3D_OK;
 }
 
 // voxel_tc.cu: sigma-only queries on the tensor cores (decoders with a density head over the shape planes, channels-last planes)
-int launch_sigma_tc(const ide3d_triplane& seg, const ide3d_decoder& dec, const float* points, long long P, int n, float box_scale,
-                    float* out, int grid_mode, int grid_n, float voxel_size, float org_x, float org_y, float org_z, float pre_scale,
-                    long long first, cudaStream_t st, bool& handled);
+int launch_sigma_tc(const VoxelArgs& a, cudaStream_t st, bool& handled);
 
 }  // namespace ide3d
 
@@ -188,7 +145,7 @@ extern "C" int ide3d_sample_voxel(const ide3d_triplane* tex, const ide3d_triplan
     a.points = points; a.P = num_points; a.box_scale = box_scale; a.sigma_only = sigma_only; a.out = out;
     if (sigma_only && cl) {
         bool handled = false;
-        rc = launch_sigma_tc(*seg, *dec, points, num_points, a.n, box_scale, out, 0, 0, 0.f, 0.f, 0.f, 0.f, 0.f, 0, (cudaStream_t)stream, handled);
+        rc = launch_sigma_tc(a, (cudaStream_t)stream, handled);
         if (handled) return rc;
     }
     return dispatch_voxel<false>(a, cl, kind, (cudaStream_t)stream);
@@ -217,8 +174,7 @@ extern "C" int ide3d_sigma_grid(const ide3d_triplane* tex, const ide3d_triplane*
     a.first = first; a.P = count; a.box_scale = box_scale; a.sigma_only = 1; a.out = out; a.points = nullptr;
     if (cl) {
         bool handled = false;
-        rc = launch_sigma_tc(*seg, *dec, nullptr, count, a.n, box_scale, out, 1, grid_n, a.voxel_size, a.org_x, a.org_y, a.org_z, pre_scale,
-                             first, (cudaStream_t)stream, handled);
+        rc = launch_sigma_tc(a, (cudaStream_t)stream, handled);
         if (handled) return rc;
     }
     return dispatch_voxel<true>(a, cl, kind, (cudaStream_t)stream);

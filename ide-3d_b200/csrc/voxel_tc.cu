@@ -14,32 +14,10 @@ namespace vtc {
 
 constexpr int kW1Bytes = 64 * 128;                                           // [64 hidden x 64 K] bf16, K columns 32..63 used
 
-struct Args {
-    PlaneView seg;
+struct Args : VoxelArgs {
     const float* w1; const float* b1; const float* w2; const float* b2;     // sigma head: [64,32], [64], [1,64], [1]
-    const float* points;           // [N, P, 3] or null (grid mode)
-    long long P;
-    int n;
-    float box_scale;
-    float* out;                    // [N, P]
-    int grid_mode, grid_n;
-    float voxel_size, org_x, org_y, org_z, pre_scale;
-    long long first;
     long long tiles_per_item, num_tiles;
 };
-
-// coordinates of flat voxel index `idx`, bit-for-bit like extract_shapes.py:74-96 followed by `0.9 *` (same arithmetic as voxel.cu)
-__device__ __forceinline__ void grid_point(const Args& a, long long idx, float& x, float& y, float& z) {
-    const float N = (float)a.grid_n;
-    const float fi = (float)idx;
-    const float s2 = (float)(idx % a.grid_n);
-    const float q1 = __fdiv_rn(fi, N);
-    const float s1 = fmodf(q1, N);
-    const float s0 = fmodf(__fdiv_rn(q1, N), N);
-    x = __fmul_rn(__fadd_rn(__fmul_rn(s0, a.voxel_size), a.org_z), a.pre_scale);
-    y = __fmul_rn(__fadd_rn(__fmul_rn(s1, a.voxel_size), a.org_y), a.pre_scale);
-    z = __fmul_rn(__fadd_rn(__fmul_rn(s2, a.voxel_size), a.org_x), a.pre_scale);
-}
 
 __global__ void __launch_bounds__(kTcThreads) sigma_tc_kernel(const Args a) {
     extern __shared__ unsigned char smem_raw[];
@@ -81,7 +59,7 @@ __global__ void __launch_bounds__(kTcThreads) sigma_tc_kernel(const Args a) {
             const long long p = p0 + l16;
             float cx = 4.f, cy = 4.f, cz = 4.f;
             if (p < a.P) {
-                if (a.grid_mode) grid_point(a, a.first + p, cx, cy, cz);
+                if (a.points == nullptr) grid_point(a, a.first + p, cx, cy, cz);
                 else { const float* pt = a.points + ((long long)n * a.P + p) * 3; cx = pt[0]; cy = pt[1]; cz = pt[2]; }
                 cx *= a.box_scale; cy *= a.box_scale; cz *= a.box_scale;
             }
@@ -141,38 +119,29 @@ __global__ void __launch_bounds__(kTcThreads) sigma_tc_kernel(const Args a) {
 
 // entry used by voxel.cu: sigma-only queries with a three-head style decoder on channels-last planes.  `handled` = false when the
 // decoder has no density head of its own over the shape planes (the CUDA-core kernel then runs).
-int launch_sigma_tc(const ide3d_triplane& seg, const ide3d_decoder& dec, const float* points, long long P, int n, float box_scale,
-                    float* out, int grid_mode, int grid_n, float voxel_size, float org_x, float org_y, float org_z, float pre_scale,
-                    long long first, cudaStream_t st, bool& handled) {
+int launch_sigma_tc(const VoxelArgs& v, cudaStream_t st, bool& handled) {
     handled = false;
     const ide3d_mlp_head* H = nullptr;
-    for (int h = 0; h < dec.num_heads; ++h) {
-        const ide3d_mlp_head& c = dec.heads[h];
+    for (int h = 0; h < v.dec.num_heads; ++h) {
+        const ide3d_mlp_head& c = v.dec.heads[h];
         if (c.out_offset <= kOut - 1 && c.out_offset + c.out_count > kOut - 1) {        // the head that produces sigma
             if (c.out_count != 1 || c.hidden != 64 || c.in_sel != 1) return IDE3D_OK;
             H = &c;
         }
     }
     if (H == nullptr) return IDE3D_OK;
-    if (((long long)seg.h * seg.stride_h + (long long)seg.w * seg.stride_w + 96) * 4 >= (1ll << 31)) return IDE3D_OK;
+    if (!plane_fits_32bit(v.seg)) return IDE3D_OK;
     if (tuning_env("IDE3D_VOXEL_SIMT") != nullptr) return IDE3D_OK;
     handled = true;
     vtc::Args a;
-    a.seg = make_view(seg);
+    static_cast<VoxelArgs&>(a) = v;
     a.w1 = H->w1; a.b1 = H->b1; a.w2 = H->w2; a.b2 = H->b2;
-    a.points = points; a.P = P; a.n = n; a.box_scale = box_scale; a.out = out;
-    a.grid_mode = grid_mode; a.grid_n = grid_n; a.voxel_size = voxel_size; a.org_x = org_x; a.org_y = org_y; a.org_z = org_z;
-    a.pre_scale = pre_scale; a.first = first;
-    a.tiles_per_item = (P + 63) / 64;
-    a.num_tiles = a.tiles_per_item * n;
+    a.tiles_per_item = (v.P + 63) / 64;
+    a.num_tiles = a.tiles_per_item * v.n;
     const int smem = 2 * vtc::kW1Bytes + kWarpgroups * kStageBytes + 128 * 4 + 1024;
-    IDE3D_CUDA(cudaFuncSetAttribute(vtc::sigma_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    int per_sm = 1;
-    IDE3D_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, vtc::sigma_tc_kernel, kTcThreads, smem));
-    if (per_sm < 1) per_sm = 1;
-    long long grid = (long long)sm_count() * per_sm;
-    if (grid * kWarpgroups > a.num_tiles) grid = (a.num_tiles + kWarpgroups - 1) / kWarpgroups;
-    vtc::sigma_tc_kernel<<<(unsigned)grid, kTcThreads, smem, st>>>(a);
+    int grid, rc;
+    if ((rc = persistent_grid(vtc::sigma_tc_kernel, kTcThreads, smem, ceil_div<long long>(a.num_tiles, kWarpgroups), grid)) != IDE3D_OK) return rc;
+    vtc::sigma_tc_kernel<<<grid, kTcThreads, smem, st>>>(a);
     IDE3D_CHECK_LAUNCH("sigma_tc_kernel");
     return IDE3D_OK;
 }

@@ -164,10 +164,12 @@ def raymarch_hierarchical(planes_tex, planes_seg, decoder, cam2world, resolution
     return (feat, depth, weights, all_z) if return_depths else (feat, depth, weights)
 
 
-def _raymarch_impl(planes_tex, planes_seg, decoder, cam2world, resolution=(64, 64), num_steps=48, fov=18.0, ray_start=2.25,
-                   ray_end=3.3, box_scale=2.0, jitter_u=None, jitter_seed=None, noise=None, noise_std=0.0,
-                   clamp_mode='softplus', last_back=False, white_back=False, max_depth=None, fill_mode=None,
-                   return_weights=False, convert_layout=True, precision='auto', z_vals=None):
+def _raymarch_params(planes_tex, planes_seg, decoder, cam2world, resolution, num_steps, fov, ray_start, ray_end, box_scale, jitter_u,
+                     jitter_seed, noise, noise_std, clamp_mode, last_back, white_back, max_depth, fill_mode, z_vals, convert_layout=True):
+    """Check the renderer options and fill the ide3d_raymarch_params that ide3d_raymarch_fwd and ide3d_raymarch_bwd share (the
+    outputs and the precision are the caller's).  S is taken from z_vals when given.
+    -> (params, tex, seg, dec, keep): `keep` holds everything the params point at (planes, packed decoder, camera, per-sample
+    tensors) and must stay referenced until the launch is enqueued, or the allocator may hand that memory to the outputs."""
     if clamp_mode not in ('softplus', 'relu'):
         raise ValueError('Need to choose clamp mode')
     if fill_mode not in (None, 'weight'):
@@ -178,33 +180,47 @@ def _raymarch_impl(planes_tex, planes_seg, decoder, cam2world, resolution=(64, 6
     dev = tex.device
     n = tex.shape[0]
     W, H = (resolution, resolution) if isinstance(resolution, int) else resolution
-    R, S = W * H, int(num_steps)
-    cam = cam2world.to(device=dev, dtype=torch.float32).reshape(n, 16).contiguous()
+    R, S = W * H, int(num_steps if z_vals is None else z_vals.shape[-1])
     dec = _decoder(decoder, dev)
-    feat = torch.empty([n, R, N_OUT - 1], dtype=torch.float32, device=dev)
-    depth = torch.empty([n, R, 1], dtype=torch.float32, device=dev)
-    weights = torch.empty([n, R, S, 1], dtype=torch.float32, device=dev) if return_weights else None
+    per_sample = lambda t: t.detach().to(device=dev, dtype=torch.float32).reshape(n, R, S).contiguous()
+    cam = cam2world.detach().to(device=dev, dtype=torch.float32).reshape(n, 16).contiguous()
+    keep = [tex, seg, dec, cam]
     p = L.RaymarchParams()
     p.tex, p.seg, p.dec = L.triplane_view(tex), L.triplane_view(seg), dec.struct
     p.cam2world = L.ptr(cam)
     p.n, p.res_w, p.res_h, p.num_steps = n, W, H, S
     p.fov_deg, p.ray_start, p.ray_end, p.box_scale = float(fov), float(ray_start), float(ray_end), float(box_scale)
     if z_vals is not None:
-        z_vals = z_vals.detach().to(device=dev, dtype=torch.float32).reshape(n, R, S).contiguous()
-        p.jitter_mode, p.jitter_u = L.JITTER_ZVALS, L.ptr(z_vals)
+        keep.append(per_sample(z_vals))
+        p.jitter_mode, p.jitter_u = L.JITTER_ZVALS, L.ptr(keep[-1])
     elif jitter_u is not None:
-        jitter_u = jitter_u.to(device=dev, dtype=torch.float32).reshape(n, R, S).contiguous()
-        p.jitter_mode, p.jitter_u = L.JITTER_TENSOR, L.ptr(jitter_u)
+        keep.append(per_sample(jitter_u))
+        p.jitter_mode, p.jitter_u = L.JITTER_TENSOR, L.ptr(keep[-1])
     elif jitter_seed is not None:
         p.jitter_mode, p.jitter_seed = L.JITTER_HASH, int(jitter_seed) & 0xFFFFFFFFFFFFFFFF
     else:
         p.jitter_mode = L.JITTER_NONE
     if noise is not None and noise_std:
-        noise = noise.to(device=dev, dtype=torch.float32).reshape(n, R, S).contiguous()
-        p.noise, p.noise_std = L.ptr(noise), float(noise_std)
+        keep.append(per_sample(noise))
+        p.noise, p.noise_std = L.ptr(keep[-1]), float(noise_std)
     p.clamp_mode = L.CLAMP_SOFTPLUS if clamp_mode == 'softplus' else L.CLAMP_RELU
     p.last_back, p.white_back = int(bool(last_back)), int(bool(white_back))
     p.max_depth, p.fill_weight = float(max_depth or 0.0), int(fill_mode == 'weight')
+    return p, tex, seg, dec, keep
+
+
+def _raymarch_impl(planes_tex, planes_seg, decoder, cam2world, resolution=(64, 64), num_steps=48, fov=18.0, ray_start=2.25,
+                   ray_end=3.3, box_scale=2.0, jitter_u=None, jitter_seed=None, noise=None, noise_std=0.0,
+                   clamp_mode='softplus', last_back=False, white_back=False, max_depth=None, fill_mode=None,
+                   return_weights=False, convert_layout=True, precision='auto', z_vals=None):
+    p, tex, _, _, keep = _raymarch_params(planes_tex, planes_seg, decoder, cam2world, resolution, num_steps, fov, ray_start, ray_end,
+                                          box_scale, jitter_u, jitter_seed, noise, noise_std, clamp_mode, last_back, white_back,
+                                          max_depth, fill_mode, z_vals, convert_layout)
+    dev = tex.device
+    n, R, S = p.n, p.res_w * p.res_h, p.num_steps
+    feat = torch.empty([n, R, N_OUT - 1], dtype=torch.float32, device=dev)
+    depth = torch.empty([n, R, 1], dtype=torch.float32, device=dev)
+    weights = torch.empty([n, R, S, 1], dtype=torch.float32, device=dev) if return_weights else None
     p.out_feat, p.out_depth, p.out_weights = L.ptr(feat), L.ptr(depth), L.ptr(weights)
     p.precision = L.PRECISION[precision]
     with torch.cuda.device(dev):
@@ -258,41 +274,17 @@ def raymarch_backward(planes_tex, planes_seg, decoder, cam2world, grad_feat, gra
     """ide3d_raymarch_bwd: gradients of (feat, depth) of `raymarch` w.r.t. the planes and the three decoder heads, one kernel that
     recomputes the per-sample chain (no materialised intermediates).  -> (d_tex | None, d_seg | None, [dW1, db1, dW2, db2] x 3 | None),
     or None when the configuration has no backward kernel (the caller then differentiates the composed chain)."""
-    L.require_cuda(planes_tex, planes_seg, cam2world, grad_feat)
-    tex, seg = as_planes(planes_tex), as_planes(planes_seg)
+    p, tex, seg, dec, keep = _raymarch_params(planes_tex, planes_seg, decoder, cam2world, resolution, num_steps, fov, ray_start, ray_end,
+                                              box_scale, jitter_u, jitter_seed, noise, noise_std, clamp_mode, last_back, white_back,
+                                              max_depth, fill_mode, z_vals)
+    L.require_cuda(grad_feat)
     dev = tex.device
-    n = tex.shape[0]
-    W, H = (resolution, resolution) if isinstance(resolution, int) else resolution
-    R, S = W * H, int(num_steps if z_vals is None else z_vals.shape[-1])
-    dec = _decoder(decoder, dev)
+    n, R, S = p.n, p.res_w * p.res_h, p.num_steps
     if dec.meta != [(0, 0), (1, N_FEAT), (1, N_FEAT + N_SEG)] or S > 256:
         return None
     shapes = [tuple(t.shape) for t in dec.tensors]
     if shapes != [(64, 32), (64,), (32, 64), (32,), (64, 32), (64,), (19, 64), (19,), (64, 32), (64,), (1, 64), (1,)]:
         return None
-    cam = cam2world.detach().to(device=dev, dtype=torch.float32).reshape(n, 16).contiguous()
-    p = L.RaymarchParams()
-    p.tex, p.seg, p.dec = L.triplane_view(tex), L.triplane_view(seg), dec.struct
-    p.cam2world = L.ptr(cam)
-    p.n, p.res_w, p.res_h, p.num_steps = n, W, H, S
-    p.fov_deg, p.ray_start, p.ray_end, p.box_scale = float(fov), float(ray_start), float(ray_end), float(box_scale)
-    keep = []
-    if z_vals is not None:
-        zt = z_vals.detach().to(device=dev, dtype=torch.float32).reshape(n, R, S).contiguous(); keep.append(zt)
-        p.jitter_mode, p.jitter_u = L.JITTER_ZVALS, L.ptr(zt)
-    elif jitter_u is not None:
-        ju = jitter_u.detach().to(device=dev, dtype=torch.float32).reshape(n, R, S).contiguous(); keep.append(ju)
-        p.jitter_mode, p.jitter_u = L.JITTER_TENSOR, L.ptr(ju)
-    elif jitter_seed is not None:
-        p.jitter_mode, p.jitter_seed = L.JITTER_HASH, int(jitter_seed) & 0xFFFFFFFFFFFFFFFF
-    else:
-        p.jitter_mode = L.JITTER_NONE
-    if noise is not None and noise_std:
-        nz = noise.detach().to(device=dev, dtype=torch.float32).reshape(n, R, S).contiguous(); keep.append(nz)
-        p.noise, p.noise_std = L.ptr(nz), float(noise_std)
-    p.clamp_mode = L.CLAMP_SOFTPLUS if clamp_mode == 'softplus' else L.CLAMP_RELU
-    p.last_back, p.white_back = int(bool(last_back)), int(bool(white_back))
-    p.max_depth, p.fill_weight = float(max_depth or 0.0), int(fill_mode == 'weight')
     gf = grad_feat.detach().to(device=dev, dtype=torch.float32).reshape(n, R, N_OUT - 1).contiguous()
     gd = None if grad_depth is None else grad_depth.detach().to(device=dev, dtype=torch.float32).reshape(n, R).contiguous()
     d_tex = torch.zeros_like(tex) if want_planes[0] else None               # channels-last, like the forward's planes

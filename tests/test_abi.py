@@ -63,6 +63,79 @@ def test_invalid_arguments_return_status_not_crash(lib):
     assert lib.ide3d_mask2color(None, 0, 19, 4, 4, 0, 0, 0, 0, None, None, 0, None) == _lib.OK                                           # empty batch
 
 
+def _fake_raymarch_params(_lib):
+    """Well-formed ide3d_raymarch_params for a 4x4 three-head render whose pointers are fake (never dereferenced)."""
+    fake = 0x10000
+    plane = lambda: _lib.TriPlane(fake, 1, 4, 4, 4 * 4 * 96, 1, 4 * 96, 96)
+    p = _lib.RaymarchParams()
+    p.tex, p.seg = plane(), plane()
+    p.dec.num_heads = 3
+    for i, (in_sel, off, cnt) in enumerate([(0, 0, 32), (1, 32, 19), (1, 51, 1)]):
+        p.dec.heads[i] = _lib.MlpHead(in_sel, 64, off, cnt, fake, fake, fake, fake)
+    p.cam2world = p.out_feat = p.out_depth = fake
+    p.n, p.res_w, p.res_h, p.num_steps = 1, 4, 4, 4
+    p.fov_deg, p.ray_start, p.ray_end, p.box_scale = 18.0, 2.25, 3.3, 2.0
+    p.jitter_mode, p.clamp_mode = _lib.JITTER_NONE, _lib.CLAMP_SOFTPLUS
+    return p
+
+
+def _set(path, value):
+    def apply(p):
+        *parents, leaf = path.split('.')
+        obj = p
+        for name in parents:
+            obj = getattr(obj, name)
+        setattr(obj, leaf, value)
+    return apply
+
+
+RAYMARCH_BROKEN = {
+    'tex null data': (_set('tex.data', None), b'tex: null data'),
+    'seg null data': (_set('seg.data', None), b'seg: null data'),
+    'seg empty': (_set('seg.h', 0), b'seg: empty tri-plane'),
+    'plane sizes differ': (_set('seg.w', 8), b'tex/seg plane sizes differ'),
+    'tex batch': (_set('tex.n', 2), b'batch mismatch'),
+    'seg batch': (_set('seg.n', 2), b'batch mismatch'),
+    'empty render': (_set('num_steps', 0), b'empty render'),
+    'null cam2world': (_set('cam2world', None), b'null camera/output'),
+    'clamp mode': (_set('clamp_mode', 7), b'Need to choose clamp mode'),
+    'jitter mode 4': (_set('jitter_mode', 4), b'bad jitter mode'),
+    'jitter mode -1': (_set('jitter_mode', -1), b'bad jitter mode'),
+    'tensor jitter missing': (_set('jitter_mode', 1), b'jitter / depth tensor missing'),
+    'z_vals missing': (_set('jitter_mode', 3), b'jitter / depth tensor missing'),
+    '2^32 samples': (lambda p: (_set('res_w', 65536)(p), _set('res_h', 65536)(p), _set('num_steps', 1)(p)), b'more than 2^32 samples'),
+}
+
+
+@pytest.mark.skipif(torch.cuda.is_available(), reason='passes fake device pointers: run only where no GPU can be reached')
+@pytest.mark.parametrize('case', sorted(RAYMARCH_BROKEN))
+def test_raymarch_entry_points_share_validation(lib, case):
+    """ide3d_raymarch_fwd and ide3d_raymarch_bwd reject the same malformed parameters with the same status and message,
+    before anything reaches the device."""
+    from ide3d_b200 import _lib
+    breaker, message = RAYMARCH_BROKEN[case]
+    p = _fake_raymarch_params(_lib)
+    breaker(p)
+    fake = ctypes.c_void_p(0x10000)
+    assert lib.ide3d_raymarch_fwd(ctypes.byref(p), None) == _lib.INVALID
+    fwd_error = lib.ide3d_last_error()
+    assert message in fwd_error
+    assert lib.ide3d_raymarch_bwd(ctypes.byref(p), fake, None, fake, fake, None, None) == _lib.INVALID
+    assert lib.ide3d_last_error() == fwd_error
+
+
+@pytest.mark.parametrize('option, error', [(dict(clamp_mode='bogus'), ValueError), (dict(fill_mode='bogus'), NotImplementedError)])
+def test_raymarch_backward_checks_options_like_forward(option, error):
+    from ide3d_b200 import render
+    planes, cam = torch.randn(1, 96, 4, 4), torch.eye(4).reshape(1, 16)
+    heads = [(0, 0, torch.zeros(64, 32), torch.zeros(64), torch.zeros(32, 64), torch.zeros(32))]
+    with pytest.raises(error) as fwd:
+        render.raymarch(planes, planes, heads, cam, resolution=4, num_steps=4, **option)
+    with pytest.raises(error) as bwd:
+        render.raymarch_backward(planes, planes, heads, cam, torch.zeros(1, 16, 51), None, resolution=4, num_steps=4, **option)
+    assert str(bwd.value) == str(fwd.value)
+
+
 def test_product_has_no_cpu_path():
     from ide3d_b200.torch_utils.ops import bias_act, filtered_lrelu, upfirdn2d
     from ide3d_b200 import render
