@@ -87,7 +87,8 @@ class RaymarchParams(C.Structure):
                 ('jitter_mode', C.c_int), ('jitter_u', C.c_void_p), ('jitter_seed', C.c_uint64),
                 ('clamp_mode', C.c_int), ('last_back', C.c_int), ('white_back', C.c_int), ('max_depth', C.c_float),
                 ('fill_weight', C.c_int), ('noise_std', C.c_float), ('noise', C.c_void_p),
-                ('out_feat', C.c_void_p), ('out_depth', C.c_void_p), ('out_weights', C.c_void_p), ('precision', C.c_int)]
+                ('out_feat', C.c_void_p), ('out_depth', C.c_void_p), ('out_weights', C.c_void_p), ('precision', C.c_int),
+                ('views', C.c_int), ('jitter_seeds', C.c_void_p)]
 
 
 class RasterParams(C.Structure):
@@ -107,6 +108,14 @@ class FramesParams(C.Structure):
                 ('seg', C.c_void_p), ('seg_c', C.c_int), ('seg_h', C.c_int), ('seg_w', C.c_int),
                 ('seg_stride_n', C.c_int64), ('seg_stride_c', C.c_int64), ('seg_stride_h', C.c_int64), ('seg_stride_w', C.c_int64),
                 ('lut', C.c_void_p), ('mode', C.c_int), ('out', C.c_void_p), ('scratch', C.c_void_p)]
+
+
+class StripsParams(C.Structure):
+    _fields_ = [('image', C.c_void_p), ('seeds', C.c_int), ('views', C.c_int), ('height', C.c_int), ('width', C.c_int),
+                ('image_stride_n', C.c_int64), ('image_stride_c', C.c_int64), ('image_stride_h', C.c_int64), ('image_stride_w', C.c_int64),
+                ('seg', C.c_void_p), ('seg_c', C.c_int), ('seg_h', C.c_int), ('seg_w', C.c_int),
+                ('seg_stride_n', C.c_int64), ('seg_stride_c', C.c_int64), ('seg_stride_h', C.c_int64), ('seg_stride_w', C.c_int64),
+                ('lut', C.c_void_p), ('out_image', C.c_void_p), ('out_seg', C.c_void_p)]
 
 
 _lib = None
@@ -182,9 +191,11 @@ def get_lib():
     lib.ide3d_raster_scratch_bytes.restype = C.c_int64
     lib.ide3d_raster.argtypes = [C.POINTER(RasterParams), vp]
     lib.ide3d_video_frames.argtypes = [C.POINTER(FramesParams), vp]
+    lib.ide3d_image_strips.argtypes = [C.POINTER(StripsParams), vp]
     for name in ('bias_act', 'upfirdn2d', 'filtered_lrelu', 'filtered_lrelu_act', 'raymarch_fwd', 'raymarch_bwd', 'sample_voxel',
                  'sigma_grid', 'planes_to_nhwc', 'initial_rays', 'transform_points', 'sample_triplane', 'integrate',
-                 'sample_pdf', 'style_plan', 'mc_classify', 'mc_emit', 'mesh_normals', 'raster', 'video_frames', 'abi_version'):
+                 'sample_pdf', 'style_plan', 'mc_classify', 'mc_emit', 'mesh_normals', 'raster', 'video_frames', 'image_strips',
+                 'abi_version'):
         getattr(lib, 'ide3d_' + name).restype = C.c_int
     if lib.ide3d_abi_version() != 1:
         raise RuntimeError('ide3d_b200: ABI version mismatch between _lib.py and libide3d_b200.so')
@@ -199,7 +210,7 @@ def exported_symbols():
             'ide3d_filtered_lrelu', 'ide3d_filtered_lrelu_act', 'ide3d_raymarch_fwd', 'ide3d_raymarch_bwd', 'ide3d_sample_voxel',
             'ide3d_sigma_grid', 'ide3d_planes_to_nhwc', 'ide3d_initial_rays', 'ide3d_transform_points',
             'ide3d_sample_triplane', 'ide3d_integrate', 'ide3d_sample_pdf', 'ide3d_mask2color', 'ide3d_style_plan', 'ide3d_mc_classify', 'ide3d_mc_emit',
-            'ide3d_mesh_normals', 'ide3d_raster_scratch_bytes', 'ide3d_raster', 'ide3d_video_frames']
+            'ide3d_mesh_normals', 'ide3d_raster_scratch_bytes', 'ide3d_raster', 'ide3d_video_frames', 'ide3d_image_strips']
 
 
 def check(rc, allow_unsupported=False):

@@ -6,7 +6,7 @@
 // Every float operation is explicitly rounded (__fmul_rn / __fadd_rn / __fsub_rn / __fdiv_rn): the reference runs each as its own torch
 // op, so a contracted FMA would round differently.  The 512^2 logits are never materialised: each pixel interpolates its classes from
 // the render-resolution logits (any strides: the strided channel view of the ray-march output is read in place).
-#include "common.cuh"
+#include "seg_common.cuh"
 
 namespace ide3d {
 
@@ -24,24 +24,6 @@ __device__ __forceinline__ unsigned char to_u8(float v) {
 __device__ __forceinline__ float nan_min(float a, float b) { return a != a ? a : (b != b ? b : fminf(a, b)); }
 __device__ __forceinline__ float nan_max(float a, float b) { return a != a ? a : (b != b ? b : fmaxf(a, b)); }
 
-// interpolate(mode='bilinear', align_corners=False) source position of output index d: max(scale * (d + 0.5) - 0.5, 0) with
-// scale = in / out; i0 = floor, i1 = i0 + 1 clamped to the last row / column, l1 = fraction.
-struct Tap {
-    int i0, i1;
-    float l0, l1;
-};
-__device__ __forceinline__ Tap bilinear_tap(int d, int in, int out) {
-    const float scale = __fdiv_rn((float)in, (float)out);
-    float s = __fsub_rn(__fmul_rn(scale, __fadd_rn((float)d, 0.5f)), 0.5f);
-    s = s < 0.f ? 0.f : s;
-    Tap t;
-    t.i0 = (int)s;
-    t.i1 = t.i0 + (t.i0 < in - 1 ? 1 : 0);
-    t.l1 = __fsub_rn(s, (float)t.i0);
-    t.l0 = __fsub_rn(1.f, t.l1);
-    return t;
-}
-
 __global__ void __launch_bounds__(kTileX * kTileY) frames_seg_kernel(ide3d_frames_params p) {
     const int x = blockIdx.x * kTileX + threadIdx.x, y = blockIdx.y * kTileY + threadIdx.y, n = blockIdx.z;
     if (x >= p.width || y >= p.height) return;
@@ -51,21 +33,9 @@ __global__ void __launch_bounds__(kTileX * kTileY) frames_seg_kernel(ide3d_frame
 #pragma unroll
     for (int c = 0; c < 3; ++c) o[c * plane] = to_u8(__ldg(im + c * p.image_stride_c));
 
-    // seg half: v = h0 * (w0 * v00 + w1 * v01) + h1 * (w0 * v10 + w1 * v11) per class, first maximum wins, NaN counts as maximal
-    const Tap ty = bilinear_tap(y, p.seg_h, p.height), tx = bilinear_tap(x, p.seg_w, p.width);
-    const float* s = p.seg + n * p.seg_stride_n;
-    const float* r0 = s + ty.i0 * p.seg_stride_h;
-    const float* r1 = s + ty.i1 * p.seg_stride_h;
-    const long long c0 = tx.i0 * p.seg_stride_w, c1 = tx.i1 * p.seg_stride_w;
-    float best = 0.f;
-    int arg = 0;
-    for (int k = 0; k < p.seg_c; ++k) {
-        const long long kc = k * p.seg_stride_c;
-        const float top = __fadd_rn(__fmul_rn(tx.l0, __ldg(r0 + kc + c0)), __fmul_rn(tx.l1, __ldg(r0 + kc + c1)));
-        const float bot = __fadd_rn(__fmul_rn(tx.l0, __ldg(r1 + kc + c0)), __fmul_rn(tx.l1, __ldg(r1 + kc + c1)));
-        const float v = __fadd_rn(__fmul_rn(ty.l0, top), __fmul_rn(ty.l1, bot));
-        if (k == 0 || v > best || (v != v && best == best)) { best = v; arg = k; }
-    }
+    // seg half: class of the bilinearly upsampled logits -> COLOR_MAP bytes
+    const int arg = seg_class_at(p.seg + n * p.seg_stride_n, p.seg_c, p.seg_h, p.seg_w, p.seg_stride_c, p.seg_stride_h, p.seg_stride_w,
+                                 x, y, p.height, p.width);
 #pragma unroll
     for (int c = 0; c < 3; ++c) o[c * plane + p.width] = (unsigned char)__ldg(p.lut + arg * 3 + c);
 }

@@ -79,9 +79,9 @@ __global__ void __launch_bounds__(kBlock, 1) raymarch_kernel(const RayArgs a) {
                     off0 = (a.jitter_u[sample_base + s] - 0.5f) * spacing;
                     if (s + 1 < S) z1 += (a.jitter_u[sample_base + s + 1] - 0.5f) * spacing;
                 } else if (a.jitter_mode == IDE3D_JITTER_HASH) {
-                    const uint32_t gi = (uint32_t)(sample_base + s);
-                    off0 = (jitter_hash(gi, a.seed_lo, a.seed_hi) - 0.5f) * spacing;
-                    if (s + 1 < S) z1 += (jitter_hash(gi + 1u, a.seed_lo, a.seed_hi) - 0.5f) * spacing;
+                    const HashKey k = hash_key(a, n, sample_base + s);
+                    off0 = (jitter_hash(k.idx, k.lo, k.hi) - 0.5f) * spacing;
+                    if (s + 1 < S) z1 += (jitter_hash(k.idx + 1u, k.lo, k.hi) - 0.5f) * spacing;
                 } else if (a.jitter_mode == IDE3D_JITTER_ZVALS) {          // depths given per sample (hierarchical second pass)
                     z0 = a.jitter_u[sample_base + s];
                     z1 = (s + 1 < S) ? a.jitter_u[sample_base + s + 1] : 0.f;
@@ -95,7 +95,7 @@ __global__ void __launch_bounds__(kBlock, 1) raymarch_kernel(const RayArgs a) {
             float cz = (m20 * pcx + m21 * pcy + m22 * pcz + m23) * a.box_scale;
             if (!live) { cx = cy = cz = 4.f; }                // far outside: every tap masked, no loads
 
-            gather_chunk<kChannelsLast>(a.tex, a.seg, n, cx, cy, cz, stage, lane);
+            gather_chunk<kChannelsLast>(a.tex, a.seg, plane_set(n, a.views), cx, cy, cz, stage, lane);
             const float* row = stage + lane * kRow;
 
             // density first: it fixes the compositing weight of this sample

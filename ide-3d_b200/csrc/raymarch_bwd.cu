@@ -39,6 +39,8 @@ struct BwdArgs {
     int clamp_mode, last_back, white_back, fill_weight;
     float max_depth, noise_std;
     const float* noise;
+    int views;                  // frames per plane set: the gradients of all views land in their shared set
+    const uint64_t* jitter_seeds;
     const float* g_feat;        // [N, R, 51]
     const float* g_depth;       // [N, R] or null
     float* g_tex;               // same layout as tex (channels-last), zero-initialised, or null
@@ -125,6 +127,7 @@ __global__ void __launch_bounds__(kBBlock, 1) raymarch_bwd_kernel(const BwdArgs 
 
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int n = tile / tiles_per_frame;
+        const int set = plane_set(n, a.views);
         const int t = tile - n * tiles_per_frame;
         const int px = (t % a.tiles_x) * kBTileX + (warp % kBTileX);
         const int py = (t / a.tiles_x) * kBTileY + (warp / kBTileX);
@@ -174,9 +177,9 @@ __global__ void __launch_bounds__(kBBlock, 1) raymarch_bwd_kernel(const BwdArgs 
                     off0 = (a.jitter_u[sample_base + s] - 0.5f) * spacing;
                     if (s + 1 < S) z1 += (a.jitter_u[sample_base + s + 1] - 0.5f) * spacing;
                 } else if (a.jitter_mode == IDE3D_JITTER_HASH) {
-                    const uint32_t gi = (uint32_t)(sample_base + s);
-                    off0 = (jitter_hash(gi, a.seed_lo, a.seed_hi) - 0.5f) * spacing;
-                    if (s + 1 < S) z1 += (jitter_hash(gi + 1u, a.seed_lo, a.seed_hi) - 0.5f) * spacing;
+                    const HashKey k = hash_key(a, n, sample_base + s);
+                    off0 = (jitter_hash(k.idx, k.lo, k.hi) - 0.5f) * spacing;
+                    if (s + 1 < S) z1 += (jitter_hash(k.idx + 1u, k.lo, k.hi) - 0.5f) * spacing;
                 } else if (a.jitter_mode == IDE3D_JITTER_ZVALS) {
                     z0 = a.jitter_u[sample_base + s];
                     z1 = (s + 1 < S) ? a.jitter_u[sample_base + s + 1] : 0.f;
@@ -197,7 +200,7 @@ __global__ void __launch_bounds__(kBBlock, 1) raymarch_bwd_kernel(const BwdArgs 
             const bool live = s < S;
             float zj, z1, cx, cy, cz;
             position(s, live, zj, z1, cx, cy, cz);
-            gather_chunk<true>(a.tex, a.seg, n, cx, cy, cz, stage, lane);
+            gather_chunk<true>(a.tex, a.seg, set, cx, cy, cz, stage, lane);
             const float* row = stage + lane * kRow;
             float q = gb + gd * zj, sigma = w2h[L2::kB2];
             {
@@ -282,7 +285,7 @@ __global__ void __launch_bounds__(kBBlock, 1) raymarch_bwd_kernel(const BwdArgs 
             const bool live = s < S;
             float zj, z1, cx, cy, cz;
             position(s, live, zj, z1, cx, cy, cz);
-            gather_chunk<true>(a.tex, a.seg, n, cx, cy, cz, stage, lane);
+            gather_chunk<true>(a.tex, a.seg, set, cx, cy, cz, stage, lane);
             float* row = stage + lane * kRow;
             const float wp = live ? s_w[s] : 0.f, ds = live ? s_q[s] : 0.f;
             wp_sum += wp; ds_sum += ds;
@@ -361,8 +364,8 @@ __global__ void __launch_bounds__(kBBlock, 1) raymarch_bwd_kernel(const BwdArgs 
                 *reinterpret_cast<float4*>(row + kFeat + k) = make_float4(df[k], df[k + 1], df[k + 2], df[k + 3]);
             }
             __syncwarp();
-            if (a.g_tex != nullptr) scatter_chunk(a.tex, a.g_tex, n, cx, cy, cz, stage, 0, lane);
-            if (a.g_seg != nullptr) scatter_chunk(a.seg, a.g_seg, n, cx, cy, cz, stage, kFeat, lane);
+            if (a.g_tex != nullptr) scatter_chunk(a.tex, a.g_tex, set, cx, cy, cz, stage, 0, lane);
+            if (a.g_seg != nullptr) scatter_chunk(a.seg, a.g_seg, set, cx, cy, cz, stage, kFeat, lane);
             __syncwarp();
         }
         if (kParams) {

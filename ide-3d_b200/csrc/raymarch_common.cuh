@@ -55,7 +55,9 @@ inline int check_raymarch_params(const ide3d_raymarch_params* p) {
     if ((rc = check_planes(p->tex, "tex")) != IDE3D_OK) return rc;
     if ((rc = check_planes(p->seg, "seg")) != IDE3D_OK) return rc;
     IDE3D_REQUIRE(p->tex.h == p->seg.h && p->tex.w == p->seg.w, "raymarch: tex/seg plane sizes differ");
-    IDE3D_REQUIRE(p->n > 0 && p->tex.n == p->n && p->seg.n == p->n, "raymarch: batch mismatch");
+    IDE3D_REQUIRE(p->views >= 0, "raymarch: negative views");
+    const long long views = p->views > 1 ? p->views : 1;
+    IDE3D_REQUIRE(p->n > 0 && (long long)p->tex.n * views == p->n && (long long)p->seg.n * views == p->n, "raymarch: batch mismatch");
     IDE3D_REQUIRE(p->res_w > 0 && p->res_h > 0 && p->num_steps > 0, "raymarch: empty render");
     IDE3D_REQUIRE(p->cam2world != nullptr, "raymarch: null camera/output");
     IDE3D_REQUIRE(p->clamp_mode == IDE3D_CLAMP_SOFTPLUS || p->clamp_mode == IDE3D_CLAMP_RELU,
@@ -81,6 +83,8 @@ struct MarchArgs {
     int clamp_mode, last_back, white_back, fill_weight;
     float max_depth, noise_std;
     const float* noise;   // null when noise_std == 0
+    int views;            // frames per plane set (>= 1)
+    const uint64_t* jitter_seeds;   // [n] per-frame HASH seeds, or null
 };
 
 // Args: MarchArgs or a struct with the same fields.  TcArgs and BwdArgs restate them instead of deriving from MarchArgs: as a
@@ -97,6 +101,33 @@ inline void fill_march_args(const ide3d_raymarch_params& p, Args& a) {
     a.clamp_mode = p.clamp_mode; a.last_back = p.last_back; a.white_back = p.white_back;
     a.fill_weight = p.fill_weight; a.max_depth = p.max_depth;
     a.noise_std = p.noise_std; a.noise = (p.noise_std != 0.f) ? p.noise : nullptr;
+    a.views = p.views > 1 ? p.views : 1;
+    a.jitter_seeds = p.jitter_seeds;
+}
+
+// The plane set frame n reads: `views` consecutive frames (the views of one latent) share one set.
+__device__ __forceinline__ int plane_set(int n, int views) { return views > 1 ? n / views : n; }
+
+// HASH jitter key of global sample index `sample` = (n * R + ray) * S + s of frame n: with per-frame seeds, jitter_seeds[n] and the
+// frame-local index (frame n is then bit-identical to a one-frame launch with that seed); otherwise the launch's seed and the global
+// index.  The hash indexes samples with 32 bits (check_raymarch_params bounds the launch).
+struct HashKey {
+    uint32_t idx, lo, hi;
+};
+template <typename Args>
+__device__ __forceinline__ HashKey hash_key(const Args& a, int n, long long sample) {
+    HashKey k;
+    if (a.jitter_seeds != nullptr) {
+        const unsigned long long seed = __ldg(reinterpret_cast<const unsigned long long*>(a.jitter_seeds) + n);
+        k.idx = (uint32_t)(sample - (long long)n * a.res_w * a.res_h * a.steps);
+        k.lo = (uint32_t)(seed & 0xffffffffull);
+        k.hi = (uint32_t)(seed >> 32);
+    } else {
+        k.idx = (uint32_t)sample;
+        k.lo = a.seed_lo;
+        k.hi = a.seed_hi;
+    }
+    return k;
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -118,8 +118,9 @@ __global__ void __launch_bounds__(kTcThreads) raymarch_tc_kernel(const TcArgs a)
         const RaySetup rA = ray_setup(a, unit, (w & 1) * 2, w >> 1);
         const RaySetup rB = ray_setup(a, unit, (w & 1) * 2 + 1, w >> 1);
         const RaySetup rG = ray_setup(a, unit, (w & 1) * 2 + (l16 >> 3), w >> 1);      // the ray of this lane's gather row
-        const char* tb = reinterpret_cast<const char*>(a.tex.base + (long long)rG.n * a.tex.sn);
-        const char* sb = reinterpret_cast<const char*>(a.seg.base + (long long)rG.n * a.seg.sn);
+        const int set = plane_set(rG.n, a.views);
+        const char* tb = reinterpret_cast<const char*>(a.tex.base + (long long)set * a.tex.sn);
+        const char* sb = reinterpret_cast<const char*>(a.seg.base + (long long)set * a.seg.sn);
         float acc[2][16];
 #pragma unroll
         for (int i = 0; i < 16; ++i) acc[0][i] = acc[1][i] = 0.f;

@@ -42,6 +42,8 @@ struct TcArgs {
     int clamp_mode, last_back, white_back, fill_weight;
     float max_depth, noise_std;
     const float* noise;
+    int views;
+    const uint64_t* jitter_seeds;
     float *out_feat, *out_depth, *out_weights;
     int units_x, units_y, num_units, tiles_per_unit;
 };
@@ -100,9 +102,9 @@ __device__ __forceinline__ void sample_depths(const TcArgs& a, const RaySetup& r
         off0 = (a.jitter_u[r.sample_base + s] - 0.5f) * r.spacing;
         if (s + 1 < S) z1 += (a.jitter_u[r.sample_base + s + 1] - 0.5f) * r.spacing;
     } else if (a.jitter_mode == IDE3D_JITTER_HASH) {
-        const uint32_t gi = (uint32_t)(r.sample_base + s);
-        off0 = (jitter_hash(gi, a.seed_lo, a.seed_hi) - 0.5f) * r.spacing;
-        if (s + 1 < S) z1 += (jitter_hash(gi + 1u, a.seed_lo, a.seed_hi) - 0.5f) * r.spacing;
+        const HashKey k = hash_key(a, r.n, r.sample_base + s);
+        off0 = (jitter_hash(k.idx, k.lo, k.hi) - 0.5f) * r.spacing;
+        if (s + 1 < S) z1 += (jitter_hash(k.idx + 1u, k.lo, k.hi) - 0.5f) * r.spacing;
     } else if (a.jitter_mode == IDE3D_JITTER_ZVALS) {                  // depths given per sample (hierarchical second pass)
         z0 = a.jitter_u[r.sample_base + s];
         z1 = (s + 1 < S) ? a.jitter_u[r.sample_base + s + 1] : 0.f;

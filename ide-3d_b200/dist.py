@@ -169,46 +169,60 @@ def stream_frames_sharded(G, ws, c, rank, world, batch=8, out=None, transport='a
         raise ValueError(f'stream_frames_sharded: image_mode must be one of {sorted(video.FRAME_WIDTH)}, got {image_mode!r}')
     width = video.FRAME_WIDTH[image_mode] * G.img_resolution
     dev = next(G.parameters()).device
+
+    def render(idx):
+        w_b, c_b = ws[idx], c[idx]
+        if image_mode == 'image_seg':
+            img, seg_raw = G.synthesis(w_b.to(dev, non_blocking=True), c=c_b.to(dev, non_blocking=True), return_seg='raw', **synthesis_kwargs)
+            return video.compose_frames(img, seg_raw, image_mode)
+        img = G.synthesis(w_b.to(dev, non_blocking=True), c=c_b.to(dev, non_blocking=True), **synthesis_kwargs)
+        if isinstance(img, (tuple, list)):
+            img = img[0]
+        if image_mode == 'image_depth':
+            return video.compose_frames(img, None, image_mode)
+        return (img * 127.5 + 128).clamp(0, 255).to(torch.uint8).contiguous()
+
+    return stream_sharded(render, F, (G.img_channels, G.img_resolution, width), dev, rank, world, batch=batch, out=out,
+                          transport=transport, tag='frames')
+
+
+def stream_sharded(render, num_items, item_shape, dev, rank, world, batch=8, out=None, transport='auto', tag='frames'):
+    """The pipeline of stream_frames_sharded for any per-item uint8 product: render(idx) -> uint8 [batch, *item_shape] on `dev` for the
+    items idx (a slice when world == 1, else an index tensor) of this rank's share i = rank, rank+world, ...; the batches reach rank 0's
+    host memory by `transport` while the next batch renders.  num_items must be a multiple of world * batch.  Returns uint8
+    [num_items, *item_shape] on the host on rank 0 (a cached buffer, or `out`), None elsewhere.  `tag` names the shared buffer."""
+    F = num_items
+    assert F % (world * batch) == 0, 'stream_sharded: the item count must be a multiple of world * batch'
     cuda = dev.type == 'cuda'
+    shape = (F,) + tuple(item_shape)
     if transport == 'auto':
         transport = 'shm' if (cuda and world > 1 and os.path.isdir('/dev/shm')) else 'nccl'
         if transport == 'shm':
             # the shared buffer must fit /dev/shm (containers often cap it): rank 0 looks, everybody follows its decision
-            shape_key = (F, G.img_channels, G.img_resolution, width)
-            need = F * G.img_channels * G.img_resolution * width
+            need = 1
+            for d in shape:
+                need *= int(d)
             ok = torch.zeros(1, dtype=torch.int32, device=dev)
-            if rank == 0 and ((shape_key, 'frames') in _shared or _shm_free_bytes() > need + (64 << 20)):
+            if rank == 0 and ((shape, tag) in _shared or _shm_free_bytes() > need + (64 << 20)):
                 ok += 1
             dist.broadcast(ok, src=0)
             if int(ok.item()) == 0:
                 transport = 'nccl'
-    shape = (F, G.img_channels, G.img_resolution, width)
     host = None
     if world > 1 and transport == 'shm':
-        host = _shared_frame_buffer(shape, rank, world, 'frames')
+        host = _shared_frame_buffer(shape, rank, world, tag)
     elif rank == 0:
         host = out if out is not None else _pinned_buffer(shape, torch.uint8)
     copy_stream = torch.cuda.Stream(dev) if cuda else None
     per_rank = F // world
     for b0 in range(0, per_rank, batch):
         if world == 1:
-            w_b, c_b = ws[b0:b0 + batch], c[b0:b0 + batch]                   # views of the pinned inputs: asynchronous H2D
+            idx = slice(b0, b0 + batch)                                      # views of the pinned inputs: asynchronous H2D
         else:
-            sel = torch.arange(rank + world * b0, rank + world * (b0 + batch), world)
-            w_b, c_b = ws[sel], c[sel]
-        if image_mode == 'image_seg':
-            img, seg_raw = G.synthesis(w_b.to(dev, non_blocking=True), c=c_b.to(dev, non_blocking=True), return_seg='raw', **synthesis_kwargs)
-            img = video.compose_frames(img, seg_raw, image_mode)
-        else:
-            img = G.synthesis(w_b.to(dev, non_blocking=True), c=c_b.to(dev, non_blocking=True), **synthesis_kwargs)
-            if isinstance(img, (tuple, list)):
-                img = img[0]
-            if image_mode == 'image_depth':
-                img = video.compose_frames(img, None, image_mode)
-            else:
-                img = (img * 127.5 + 128).clamp(0, 255).to(torch.uint8).contiguous()
+            idx = torch.arange(rank + world * b0, rank + world * (b0 + batch), world)
+        img = render(idx)
         if world > 1 and transport == 'shm':
-            # my frames k of this batch are global frames rank + world * (b0 + k): one asynchronous copy per frame into the shared buffer
+            # my items k of this batch are global items rank + world * (b0 + k): one asynchronous copy per item into the shared buffer
             if cuda:
                 copy_stream.wait_stream(torch.cuda.current_stream(dev))
                 with torch.cuda.stream(copy_stream):
@@ -222,7 +236,7 @@ def stream_frames_sharded(G, ws, c, rank, world, batch=8, out=None, transport='a
         if world > 1:
             allf = torch.empty((world,) + tuple(img.shape), dtype=img.dtype, device=dev)
             dist.all_gather_into_tensor(allf.view((world * img.shape[0],) + tuple(img.shape[1:])), img)
-            img = allf.transpose(0, 1).reshape((world * batch,) + tuple(img.shape[1:]))     # frame order: j * world + r
+            img = allf.transpose(0, 1).reshape((world * batch,) + tuple(img.shape[1:]))     # item order: j * world + r
         if rank == 0:
             lo = world * b0
             if cuda:
@@ -237,7 +251,7 @@ def stream_frames_sharded(G, ws, c, rank, world, batch=8, out=None, transport='a
             copy_stream.synchronize()
         torch.cuda.current_stream(dev).synchronize()
     if world > 1 and transport == 'shm':
-        dist.barrier()                                   # every rank's frames are in the shared buffer
+        dist.barrier()                                   # every rank's items are in the shared buffer
         if rank != 0:
             return None
         if out is not None:

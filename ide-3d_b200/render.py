@@ -6,6 +6,7 @@ Everything takes CUDA tensors and raises otherwise.  The decoder is passed as a 
 """
 
 import ctypes as C
+import numbers
 
 import torch
 
@@ -61,19 +62,43 @@ def _decoder(dec, device):
     return dec if isinstance(dec, PackedDecoder) else PackedDecoder(dec, device)
 
 
+def frame_seeds(jitter_seed):
+    """The per-frame form of a `jitter_seed` argument: None for an int (one seed for the launch) or None, else the list of per-frame
+    seeds given as a sequence or a 1-D integer tensor."""
+    if jitter_seed is None or isinstance(jitter_seed, numbers.Integral):
+        return None
+    if isinstance(jitter_seed, torch.Tensor):
+        if jitter_seed.ndim == 0:
+            return None
+        if jitter_seed.ndim != 1 or jitter_seed.is_floating_point():
+            raise ValueError('ide3d_b200.render: per-frame jitter seeds must be a 1-D integer tensor')
+        return [int(v) for v in jitter_seed.tolist()]
+    return [int(v) for v in jitter_seed]
+
+
+def _seed_array(seeds, device):
+    """uint64 seeds as the int64 device array the kernel reads (same bits)."""
+    m = 0xFFFFFFFFFFFFFFFF
+    return torch.tensor([(v & m) - (1 << 64) if (v & m) >= (1 << 63) else (v & m) for v in seeds], dtype=torch.int64, device=device)
+
+
 def raymarch(planes_tex, planes_seg, decoder, cam2world, resolution=(64, 64), num_steps=48, fov=18.0, ray_start=2.25,
              ray_end=3.3, box_scale=2.0, jitter_u=None, jitter_seed=None, noise=None, noise_std=0.0,
              clamp_mode='softplus', last_back=False, white_back=False, max_depth=None, fill_mode=None,
-             return_weights=False, convert_layout=True, precision='auto', z_vals=None):
+             return_weights=False, convert_layout=True, precision='auto', z_vals=None, views=1):
     """Fused render of N frames.  -> feat [N,R,51], depth [N,R,1], weights [N,R,S,1] | None.
-    jitter_u: explicit uniforms [N,R,S]; jitter_seed: in-kernel counter hash; neither: no jitter.
+    views: frames per plane set -- the planes hold N / views sets and frame f reads set f // views (the views of one latent share
+    its planes); cam2world and the per-sample tensors have N rows.
+    jitter_u: explicit uniforms [N,R,S]; jitter_seed: in-kernel counter hash, one int for the launch, or a sequence / 1-D integer
+    tensor of N per-frame seeds (frame f then jitters exactly as a one-frame launch with seed jitter_seed[f]); neither: no jitter.
     z_vals: explicit sample depths [N,R,S] ascending along S (replaces linspace + jitter; num_steps is taken from it).
     precision: 'auto' | 'fp32' (CUDA-core FFMA decoder) | 'tc' (wgmma tensor-core decoder, bf16x3 products).
     Differentiable w.r.t. the planes, the camera and the decoder parameters (when `decoder` is a list of heads holding the
     live parameters): the forward is the same fused kernel, the backward is render_grad.RaymarchFunction."""
     kw = dict(resolution=resolution, num_steps=num_steps, fov=fov, ray_start=ray_start, ray_end=ray_end, box_scale=box_scale,
               jitter_seed=jitter_seed, noise_std=noise_std, clamp_mode=clamp_mode, last_back=last_back, white_back=white_back,
-              max_depth=max_depth, fill_mode=fill_mode, return_weights=return_weights, convert_layout=convert_layout, precision=precision)
+              max_depth=max_depth, fill_mode=fill_mode, return_weights=return_weights, convert_layout=convert_layout, precision=precision,
+              views=views)
     if z_vals is not None:
         if torch.is_grad_enabled() and z_vals.requires_grad:
             raise RuntimeError('ide3d_b200.render.raymarch: z_vals is not differentiable (the reference detaches the importance samples too)')
@@ -93,12 +118,12 @@ def raymarch(planes_tex, planes_seg, decoder, cam2world, resolution=(64, 64), nu
         cfg = dict(W=int(W), H=int(H), S=int(num_steps), fov=float(fov), ray_start=float(ray_start), ray_end=float(ray_end),
                    box_scale=float(box_scale), jitter_seed=None if jitter_u is not None else jitter_seed, noise_std=float(noise_std or 0.0),
                    clamp_mode=clamp_mode, last_back=bool(last_back), white_back=bool(white_back), max_depth=float(max_depth or 0.0),
-                   fill_weight=(fill_mode == 'weight'))
+                   fill_weight=(fill_mode == 'weight'), views=int(views))
 
         def fwd(tex, seg, heads, cam, ju, nz):
             return _raymarch_impl(tex, seg, heads, cam, jitter_u=ju, noise=nz, **kw)
 
-        n = planes_tex.shape[0]
+        n = planes_tex.shape[0] * max(int(views), 1)
         feat, depth, weights = render_grad.RaymarchFunction.apply(fwd, cfg, meta, jitter_u, noise, bool(return_weights), planes_tex.float(),
                                                                   planes_seg.float(), cam2world.reshape(n, 4, 4).float(), *params)
         return feat, depth, (weights if return_weights else None)
@@ -107,14 +132,18 @@ def raymarch(planes_tex, planes_seg, decoder, cam2world, resolution=(64, 64), nu
 
 def coarse_depths(n, resolution, num_steps, ray_start=2.25, ray_end=3.3, jitter_u=None, jitter_seed=None, device='cuda'):
     """z_vals [N, R, S] of the first (stratified) pass exactly as the fused kernel generates them: torch.linspace(ray_start, ray_end, S)
-    (volumetric_rendering.py:91) + (u - 0.5) * (z[1] - z[0]) (:99-105), u = jitter_u or the kernel's counter hash."""
+    (volumetric_rendering.py:91) + (u - 0.5) * (z[1] - z[0]) (:99-105), u = jitter_u or the kernel's counter hash (one seed, or n
+    per-frame seeds as render.raymarch takes them)."""
     W, H = (resolution, resolution) if isinstance(resolution, int) else resolution
     R, S = W * H, int(num_steps)
     z = torch.linspace(ray_start, ray_end, S, device=device, dtype=torch.float32)
     zv = z.reshape(1, 1, S).expand(n, R, S)
     if jitter_u is None and jitter_seed is not None:
-        from .render_grad import hash_uniform
-        jitter_u = hash_uniform(n * R * S, jitter_seed, device)
+        from .render_grad import hash_uniform, hash_uniform_frames
+        seeds = frame_seeds(jitter_seed)
+        if seeds is not None and len(seeds) != n:
+            raise ValueError(f'ide3d_b200.render.coarse_depths: {len(seeds)} per-frame seeds for {n} frames')
+        jitter_u = hash_uniform(n * R * S, jitter_seed, device) if seeds is None else hash_uniform_frames(R * S, seeds, device)
     if jitter_u is None:
         return zv.contiguous()
     spacing = (z[1] - z[0]) if S > 1 else z.new_zeros(())
@@ -124,7 +153,7 @@ def coarse_depths(n, resolution, num_steps, ray_start=2.25, ray_end=3.3, jitter_
 @torch.no_grad()
 def raymarch_hierarchical(planes_tex, planes_seg, decoder, cam2world, resolution=(64, 64), num_steps=48, n_importance=None,
                           ray_start=2.25, ray_end=3.3, jitter_u=None, jitter_seed=None, importance_u=None, det=False,
-                          return_weights=False, return_depths=False, **kw):
+                          return_weights=False, return_depths=False, views=1, **kw):
     """Two-pass (coarse -> importance) render, the hierarchical sampling that `sample_pdf` exists for
     (volumetric_rendering.py:224-265; used as in pi-GAN / StyleNeRF's renderers, dnnlib/camera.py:638):
         1. coarse fused pass over the stratified depths, returning the compositing weights;
@@ -132,11 +161,12 @@ def raymarch_hierarchical(planes_tex, planes_seg, decoder, cam2world, resolution
            midpoints of the coarse depths (importance_u [N*R, n_importance] injects the uniform draws; det=True uses linspace);
         3. the coarse and fine depths merged and sorted per ray; second fused pass over all S + n_importance samples with the depths
            read from that tensor (IDE3D_JITTER_ZVALS) -- compositing over the merged set, as the reference composition does.
+    views, jitter_seed: as in `raymarch` (N = planes * views frames).
     Forward only.  -> feat [N,R,51], depth [N,R,1], weights [N,R,S+n_importance,1] | None (, z_vals [N,R,S+n_importance])."""
     from .training.volumetric_rendering import sample_pdf_u
     L.require_cuda(planes_tex, planes_seg, cam2world)
     dev = planes_tex.device
-    n = planes_tex.shape[0]
+    n = planes_tex.shape[0] * max(int(views), 1)
     W, H = (resolution, resolution) if isinstance(resolution, int) else resolution
     R, S = W * H, int(num_steps)
     n_imp = S if n_importance is None else int(n_importance)
@@ -144,7 +174,7 @@ def raymarch_hierarchical(planes_tex, planes_seg, decoder, cam2world, resolution
     tex, seg = as_planes(planes_tex), as_planes(planes_seg)
     dec = _decoder(decoder, dev)
     z = coarse_depths(n, (W, H), S, ray_start, ray_end, jitter_u=jitter_u, jitter_seed=jitter_seed, device=dev)
-    kw = dict(kw, convert_layout=False)
+    kw = dict(kw, convert_layout=False, views=views)
     noise_std = float(kw.pop('noise_std', 0.0) or 0.0)
     kw.pop('noise', None)                                  # drawn per pass (the two passes have different sample counts)
     draw = (lambda s_: dict(noise=torch.randn(n, R, s_, device=dev), noise_std=noise_std)) if noise_std else (lambda s_: {})
@@ -165,7 +195,8 @@ def raymarch_hierarchical(planes_tex, planes_seg, decoder, cam2world, resolution
 
 
 def _raymarch_params(planes_tex, planes_seg, decoder, cam2world, resolution, num_steps, fov, ray_start, ray_end, box_scale, jitter_u,
-                     jitter_seed, noise, noise_std, clamp_mode, last_back, white_back, max_depth, fill_mode, z_vals, convert_layout=True):
+                     jitter_seed, noise, noise_std, clamp_mode, last_back, white_back, max_depth, fill_mode, z_vals, convert_layout=True,
+                     views=1):
     """Check the renderer options and fill the ide3d_raymarch_params that ide3d_raymarch_fwd and ide3d_raymarch_bwd share (the
     outputs and the precision are the caller's).  S is taken from z_vals when given.
     -> (params, tex, seg, dec, keep): `keep` holds everything the params point at (planes, packed decoder, camera, per-sample
@@ -178,7 +209,10 @@ def _raymarch_params(planes_tex, planes_seg, decoder, cam2world, resolution, num
     tex = as_planes(planes_tex) if convert_layout else planes_tex
     seg = as_planes(planes_seg) if convert_layout else planes_seg
     dev = tex.device
-    n = tex.shape[0]
+    views = int(views)
+    if views < 1:
+        raise ValueError(f'ide3d_b200.render: views must be >= 1, got {views}')
+    n = tex.shape[0] * views                                                 # frames
     W, H = (resolution, resolution) if isinstance(resolution, int) else resolution
     R, S = W * H, int(num_steps if z_vals is None else z_vals.shape[-1])
     dec = _decoder(decoder, dev)
@@ -188,7 +222,7 @@ def _raymarch_params(planes_tex, planes_seg, decoder, cam2world, resolution, num
     p = L.RaymarchParams()
     p.tex, p.seg, p.dec = L.triplane_view(tex), L.triplane_view(seg), dec.struct
     p.cam2world = L.ptr(cam)
-    p.n, p.res_w, p.res_h, p.num_steps = n, W, H, S
+    p.n, p.res_w, p.res_h, p.num_steps, p.views = n, W, H, S, views
     p.fov_deg, p.ray_start, p.ray_end, p.box_scale = float(fov), float(ray_start), float(ray_end), float(box_scale)
     if z_vals is not None:
         keep.append(per_sample(z_vals))
@@ -197,7 +231,14 @@ def _raymarch_params(planes_tex, planes_seg, decoder, cam2world, resolution, num
         keep.append(per_sample(jitter_u))
         p.jitter_mode, p.jitter_u = L.JITTER_TENSOR, L.ptr(keep[-1])
     elif jitter_seed is not None:
-        p.jitter_mode, p.jitter_seed = L.JITTER_HASH, int(jitter_seed) & 0xFFFFFFFFFFFFFFFF
+        seeds = frame_seeds(jitter_seed)
+        if seeds is None:
+            p.jitter_mode, p.jitter_seed = L.JITTER_HASH, int(jitter_seed) & 0xFFFFFFFFFFFFFFFF
+        else:
+            if len(seeds) != n:
+                raise ValueError(f'ide3d_b200.render: {len(seeds)} per-frame jitter seeds for {n} frames')
+            keep.append(_seed_array(seeds, dev))
+            p.jitter_mode, p.jitter_seeds = L.JITTER_HASH, L.ptr(keep[-1])
     else:
         p.jitter_mode = L.JITTER_NONE
     if noise is not None and noise_std:
@@ -212,10 +253,10 @@ def _raymarch_params(planes_tex, planes_seg, decoder, cam2world, resolution, num
 def _raymarch_impl(planes_tex, planes_seg, decoder, cam2world, resolution=(64, 64), num_steps=48, fov=18.0, ray_start=2.25,
                    ray_end=3.3, box_scale=2.0, jitter_u=None, jitter_seed=None, noise=None, noise_std=0.0,
                    clamp_mode='softplus', last_back=False, white_back=False, max_depth=None, fill_mode=None,
-                   return_weights=False, convert_layout=True, precision='auto', z_vals=None):
+                   return_weights=False, convert_layout=True, precision='auto', z_vals=None, views=1):
     p, tex, _, _, keep = _raymarch_params(planes_tex, planes_seg, decoder, cam2world, resolution, num_steps, fov, ray_start, ray_end,
                                           box_scale, jitter_u, jitter_seed, noise, noise_std, clamp_mode, last_back, white_back,
-                                          max_depth, fill_mode, z_vals, convert_layout)
+                                          max_depth, fill_mode, z_vals, convert_layout, views)
     dev = tex.device
     n, R, S = p.n, p.res_w * p.res_h, p.num_steps
     feat = torch.empty([n, R, N_OUT - 1], dtype=torch.float32, device=dev)
@@ -270,13 +311,14 @@ def sigma_grid(planes_tex, planes_seg, decoder, grid_n=256, voxel_origin=(0, 0, 
 def raymarch_backward(planes_tex, planes_seg, decoder, cam2world, grad_feat, grad_depth, resolution=(64, 64), num_steps=48, fov=18.0,
                       ray_start=2.25, ray_end=3.3, box_scale=2.0, jitter_u=None, jitter_seed=None, noise=None, noise_std=0.0,
                       clamp_mode='softplus', last_back=False, white_back=False, max_depth=None, fill_mode=None, z_vals=None,
-                      want_planes=(True, True), want_params=True):
+                      want_planes=(True, True), want_params=True, views=1):
     """ide3d_raymarch_bwd: gradients of (feat, depth) of `raymarch` w.r.t. the planes and the three decoder heads, one kernel that
     recomputes the per-sample chain (no materialised intermediates).  -> (d_tex | None, d_seg | None, [dW1, db1, dW2, db2] x 3 | None),
-    or None when the configuration has no backward kernel (the caller then differentiates the composed chain)."""
+    or None when the configuration has no backward kernel (the caller then differentiates the composed chain).
+    views: as in `raymarch`; the plane gradients of all views of a plane set accumulate into that set's gradient."""
     p, tex, seg, dec, keep = _raymarch_params(planes_tex, planes_seg, decoder, cam2world, resolution, num_steps, fov, ray_start, ray_end,
                                               box_scale, jitter_u, jitter_seed, noise, noise_std, clamp_mode, last_back, white_back,
-                                              max_depth, fill_mode, z_vals)
+                                              max_depth, fill_mode, z_vals, views=views)
     L.require_cuda(grad_feat)
     dev = tex.device
     n, R, S = p.n, p.res_w * p.res_h, p.num_steps

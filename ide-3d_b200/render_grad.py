@@ -37,6 +37,12 @@ def hash_uniform(count, seed, device, first=0):
     return (h >> 8).to(torch.float32) * (1.0 / 16777216.0)
 
 
+def hash_uniform_frames(count, seeds, device, first=0):
+    """Per-frame twin of hash_uniform (the kernel's per-frame seed mode, ide3d_raymarch_params.jitter_seeds): row f holds the uniforms
+    of the frame-local sample indices first .. first+count-1 hashed with seeds[f].  -> [len(seeds), count]"""
+    return torch.stack([hash_uniform(count, s, device, first) for s in seeds]) if len(seeds) else torch.empty(0, count, device=device)
+
+
 def _gather(coords, planes):
     """sample_from_triplane: planes [n,96,H,W], coords [n,P,3] in grid units -> [n,P,32] (sum over xy, yz, xz)."""
     n, c3, h, w = planes.shape
@@ -60,8 +66,13 @@ def _decode(f_tex, f_seg, heads):
 
 def composed_chain(tex, seg, heads, cam2world, cfg, jitter_u=None, noise=None, rays=None):
     """The renderer chain on materialised tensors.  tex/seg [n,96,H,W]; cam2world [n,4,4]; cfg: dict(W, H, S, fov, ray_start,
-    ray_end, box_scale, jitter_seed, noise_std, clamp_mode, last_back, white_back, max_depth, fill_weight).
+    ray_end, box_scale, jitter_seed, noise_std, clamp_mode, last_back, white_back, max_depth, fill_weight[, views]).
+    views > 1: the planes hold n / views sets, frame f reads set f // views (materialised here by repeat_interleave, so autograd sums
+    the views' gradients into their set); jitter_seed may be a list of per-frame seeds.
     rays: optional (first, count) slab of the R = W*H rays.  -> feat [n,r,51], depth [n,r,1], weights [n,r,S,1]."""
+    views = int(cfg.get('views', 1) or 1)
+    if views > 1:
+        tex, seg = tex.repeat_interleave(views, 0), seg.repeat_interleave(views, 0)
     dev = tex.device
     n = tex.shape[0]
     W, H, S = cfg['W'], cfg['H'], cfg['S']
@@ -80,7 +91,12 @@ def composed_chain(tex, seg, heads, cam2world, cfg, jitter_u=None, noise=None, r
     if jitter_u is not None:
         u = jitter_u.reshape(n, R, S)[:, r0:r0 + rc]
     elif cfg.get('jitter_seed') is not None:
-        u = torch.stack([hash_uniform(rc * S, cfg['jitter_seed'], dev, first=(i * R + r0) * S).reshape(rc, S) for i in range(n)])
+        from .render import frame_seeds
+        seeds = frame_seeds(cfg['jitter_seed'])
+        if seeds is None:
+            u = torch.stack([hash_uniform(rc * S, cfg['jitter_seed'], dev, first=(i * R + r0) * S).reshape(rc, S) for i in range(n)])
+        else:
+            u = hash_uniform_frames(rc * S, seeds, dev, first=r0 * S).reshape(n, rc, S)
     if u is not None and S > 1:
         z_vals = z_vals + (u - 0.5) * (zv[1] - zv[0])
     pts = d.reshape(1, rc, 1, 3) * z_vals.unsqueeze(-1)                      # camera space
@@ -139,7 +155,7 @@ class RaymarchFunction(torch.autograd.Function):
             kw = dict(resolution=(cfg['W'], cfg['H']), num_steps=cfg['S'], fov=cfg['fov'], ray_start=cfg['ray_start'], ray_end=cfg['ray_end'],
                       box_scale=cfg['box_scale'], jitter_u=jitter_u, jitter_seed=cfg.get('jitter_seed'), noise=noise, noise_std=cfg.get('noise_std', 0.0),
                       clamp_mode=cfg['clamp_mode'], last_back=cfg['last_back'], white_back=cfg['white_back'], max_depth=cfg['max_depth'],
-                      fill_mode='weight' if cfg['fill_weight'] else None)
+                      fill_mode='weight' if cfg['fill_weight'] else None, views=cfg.get('views', 1))
             res = render.raymarch_backward(tex, seg, heads, cam2world, dfeat, ddepth, want_planes=(bool(need[0]), bool(need[1])),
                                            want_params=any(need[3:]), **kw)
             if res is not None:

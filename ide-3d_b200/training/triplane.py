@@ -103,14 +103,16 @@ class TriPlaneRenderer(torch.nn.Module):
     def forward(self, img_v, seg_v, cam2world, img_size=64, num_steps=48, fov=18.0, ray_start=2.25, ray_end=3.3,
                 nerf_noise=0.0, perturb='hash', jitter_u=None, seed=None, clamp_mode='softplus', last_back=False,
                 white_back=False, max_depth=None, fill_mode=None, return_weights=False, hierarchical=False, n_importance=None,
-                importance_u=None):
+                importance_u=None, views=1):
         """-> feat [N, R, 51] (32 colour + 19 semantic), depth [N, R, 1], weights [N, R, S, 1] | None.
+        views: frames per plane set; img_v / seg_v hold N / views sets and cam2world N rows, view j of set i being frame
+        i * views + j.  seed: one int, or N per-frame seeds (frame f then jitters as a one-frame call with seed[f]).
         hierarchical: two-pass importance sampling (render.raymarch_hierarchical; sample_pdf, volumetric_rendering.py:224-265) with
         n_importance (default num_steps) extra samples per ray; forward only.  Off by default: whether the released generator samples
         hierarchically is not recoverable from the reference tree (SURVEY.md a8).
         perturb: 'hash' (in-kernel counter hash seeded from torch's CPU generator), 'rand' (torch.rand on the device,
         the draw the reference makes at volumetric_rendering.py:101), or None/False (no jitter)."""
-        n = img_v.shape[0]
+        n = img_v.shape[0] * views
         res = (img_size, img_size) if isinstance(img_size, int) else tuple(img_size)
         if jitter_u is None and perturb == 'rand':
             jitter_u = torch.rand([n, res[0] * res[1], num_steps], device=img_v.device)
@@ -129,12 +131,12 @@ class TriPlaneRenderer(torch.nn.Module):
                                                 box_scale=self.box_scale, jitter_u=jitter_u, jitter_seed=seed, importance_u=importance_u,
                                                 det=perturb in (None, False, 'none'), noise_std=float(nerf_noise or 0.0),
                                                 clamp_mode=clamp_mode, last_back=last_back, white_back=white_back, max_depth=max_depth,
-                                                fill_mode=fill_mode, return_weights=return_weights)
+                                                fill_mode=fill_mode, return_weights=return_weights, views=views)
         return render.raymarch(img_v, seg_v, self.heads() if train else self.packed(), cam2world, resolution=res, num_steps=num_steps, fov=fov,
                                ray_start=ray_start, ray_end=ray_end, box_scale=self.box_scale, jitter_u=jitter_u,
                                jitter_seed=seed, noise=noise, noise_std=float(nerf_noise or 0.0), clamp_mode=clamp_mode,
                                last_back=last_back, white_back=white_back, max_depth=max_depth, fill_mode=fill_mode,
-                               return_weights=return_weights)
+                               return_weights=return_weights, views=views)
 
 
 # ================================================================================================ synthesis
@@ -234,21 +236,37 @@ class SynthesisNetwork(torch.nn.Module):
         return rgb
 
     def forward(self, ws, c=None, render_params=None, noise_mode='const', force_fp32=False, return_seg=False,
-                return_raw=False, return_dict=False, fused_modconv=None, **render_overrides):
+                return_raw=False, return_dict=False, fused_modconv=None, views=1, **render_overrides):
+        """views (extension): render every latent from `views` cameras with ONE backbone pass.  ws [N, num_ws, w_dim]; c [N * views, 25]
+        in latent-major order (row i * views + j is view j of latent i); every output has N * views rows in that order.  The
+        tri-plane backbone runs on the N latents, the renderer and the super-resolution blocks per view (their ws repeated per view).
+        seed= (a render override) may then hold N * views per-frame jitter seeds."""
+        views = int(views)
+        if views < 1:
+            raise ValueError(f'SynthesisNetwork: views must be >= 1, got {views}')
         voxel_ws, block_ws = self.split_ws(ws)
         block_kwargs = dict(noise_mode=noise_mode, force_fp32=force_fp32, fused_modconv=fused_modconv)
         plan = self._style_plan(ws)
         if plan is not None:
             block_kwargs['style_plan'] = plan
         img_v, seg_v = self.backbone(voxel_ws, **block_kwargs)
+        if views > 1:
+            # the per-view part: SR styles are functions of the ws row alone, so the plan's rows are repeated rather than recomputed
+            block_ws = [w.repeat_interleave(views, 0) for w in block_ws]
+            if plan is not None:
+                rep = lambda t: None if t is None else t.repeat_interleave(views, 0)
+                sr_layers = {m for r in self.block_resolutions for m in getattr(self, f'b{r}').modules()}
+                block_kwargs['style_plan'] = {layer: (rep(st), rep(dc)) for layer, (st, dc) in plan.items() if layer in sr_layers}
 
         kw = dict(self.rendering_kwargs)
         kw.update({k: v for k, v in (render_params or {}).items() if k in ('fov', 'num_steps', 'ray_start', 'ray_end',
                                                                           'nerf_noise', 'white_back', 'last_back',
                                                                           'clamp_mode', 'perturb', 'hierarchical', 'n_importance')})
         kw.update(render_overrides)
-        n = ws.shape[0]
+        n = ws.shape[0] * views
         if c is not None:
+            if views > 1 and c.shape[0] != n:
+                raise ValueError(f'SynthesisNetwork: c has {c.shape[0]} rows, expected ws rows x views = {n}')
             cam2world = c[:, :16].reshape(-1, 4, 4)
         else:   # no label: build the pose from the render params' means (frontal by default)
             from .volumetric_rendering import create_cam2world_matrix, sample_camera_positions
@@ -258,6 +276,8 @@ class SynthesisNetwork(torch.nn.Module):
                                                    vertical_mean=rp.get('v_mean', math.pi / 2), mode=None)
             cam2world = create_cam2world_matrix(-origin, origin, device=ws.device)
         R = self.render_size
+        if views > 1:
+            kw['views'] = views
         feat, depth, _ = self.renderer(img_v, seg_v, cam2world, img_size=R, **kw)
         maps = feat.permute(0, 2, 1).reshape(n, N_OUT - 1, R, R)
         # feat is [N, HW, 51]: already channels-last; keep that layout for the super-resolution blocks when they use it

@@ -18,6 +18,7 @@
  *   ide3d_sample_pdf          training/volumetric_rendering.py:224  sample_pdf
  *   ide3d_mask2color          dnnlib/seg_tools.py:75                mask2color
  *   ide3d_video_frames        gen_videos.py:129-139 + layout_grid :24-38  image_seg / image_depth frames, fused
+ *   ide3d_image_strips        gen_images.py:109-116  mask2color + the two save_image strips (make_grid + uint8), fused
  *   ide3d_sample_voxel        generator.synthesis.renderer.sample_voxel (call site extract_shapes.py:146)
  *   ide3d_sigma_grid          extract_shapes.py:99-150 (create_samples :74-96 + the sample_voxel loop :144-148)
  *   ide3d_raymarch_fwd        the per-frame chain the generator class runs: rays -> jitter -> world
@@ -241,6 +242,10 @@ typedef struct ide3d_raymarch_params {
     float* out_depth;           /* [N, R] */
     float* out_weights;         /* [N, R, S] or NULL */
     int precision;              /* ide3d_precision: how the decoder MLP is evaluated */
+    int views;                  /* frames per plane set: frame f reads plane set f / views (tex.n == seg.n == n / views);
+                                   0 or 1: one plane set per frame */
+    const uint64_t* jitter_seeds; /* [n] device array or NULL.  HASH jitter of frame f then uses jitter_seeds[f] and the frame-local
+                                   sample index, so frame f equals a one-frame launch with jitter_seed = jitter_seeds[f] */
 } ide3d_raymarch_params;
 int ide3d_raymarch_fwd(const ide3d_raymarch_params* p, ide3d_stream_t stream);
 
@@ -332,6 +337,31 @@ typedef struct ide3d_frames_params {
     float* scratch;             /* IMAGE_DEPTH only */
 } ide3d_frames_params;
 int ide3d_video_frames(const ide3d_frames_params* p, ide3d_stream_t stream);
+
+/* The two PNG strips gen_images.py writes per seed (gen_images.py:109-116), in the uint8 HWC form PIL saves, straight from the synthesis
+ * outputs of its `views` yaws:
+ *   image [seeds * views, 3, height, width] fp32, element strides; row s * views + j is view j of seed s.
+ *   seg   [seeds * views, seg_c, seg_h, seg_w] fp32, element strides: the render-resolution logits, upsampled per pixel to height x width
+ *         by interpolate(mode='bilinear', align_corners=False) and never stored.  lut [seg_c, 3] fp32 (the COLOR_MAP rows).
+ *   out_image, out_seg: dense uint8 [seeds, strip_h, strip_w, 3].
+ * Strip layout: torchvision's make_grid(nrow=8, padding=2, pad_value=0), one row of views (views <= 8): strip_h = height + 4,
+ * strip_w = views * (width + 2) + 2, view j at row 2, column 2 + j * (width + 2), padding bytes 0; views == 1: the bare image
+ * (strip_h = height, strip_w = width).
+ * Image bytes: save_image(normalize=True, value_range=(-1, 1)): clamp(x, -1, 1) - (-1), / 2, * 255, + 0.5, clamp(0, 255), -> uint8, each
+ * operation rounded separately; NaN gets the byte torch's device conversion writes.  Seg bytes: the COLOR_MAP bytes of the argmax class
+ * (first maximum, NaN maximal) -- the save_image chain of (colour / 255 - 0.5) / 0.5 gives the colour back exactly.  Limits: seeds <= 65535. */
+typedef struct ide3d_strips_params {
+    const float* image;
+    int seeds, views, height, width;
+    int64_t image_stride_n, image_stride_c, image_stride_h, image_stride_w;
+    const float* seg;
+    int seg_c, seg_h, seg_w;
+    int64_t seg_stride_n, seg_stride_c, seg_stride_h, seg_stride_w;
+    const float* lut;
+    uint8_t* out_image;
+    uint8_t* out_seg;
+} ide3d_strips_params;
+int ide3d_image_strips(const ide3d_strips_params* p, ide3d_stream_t stream);
 
 /* Marching cubes on a density grid (render_mesh.py:30-32 / dnnlib/geometry.py:282-286 call PyMCubes' marching_cubes on the host).
  * volume [nx, ny, nz] fp32 dense (index (x*ny + y)*nz + z); a corner is inside where value >= threshold.  Tables (device memory) come
