@@ -173,6 +173,7 @@ def get_lib():
     lib.ide3d_filtered_lrelu_act.argtypes = [C.POINTER(FlreluActParams), vp]
     lib.ide3d_raymarch_fwd.argtypes = [C.POINTER(RaymarchParams), vp]
     lib.ide3d_raymarch_bwd.argtypes = [C.POINTER(RaymarchParams), vp, vp, vp, vp, C.POINTER(C.c_void_p), vp]
+    lib.ide3d_raymarch_bwd_cam.argtypes = [C.POINTER(RaymarchParams), vp, vp, vp, vp, C.POINTER(C.c_void_p), vp, vp]
     lib.ide3d_sample_voxel.argtypes = [C.POINTER(TriPlane), C.POINTER(TriPlane), C.POINTER(Decoder), vp, i64, f32, i32, vp, vp]
     lib.ide3d_sigma_grid.argtypes = [C.POINTER(TriPlane), C.POINTER(TriPlane), C.POINTER(Decoder), i32,
                                      C.POINTER(C.c_float * 3), f32, f32, f32, i64, i64, vp, vp]
@@ -192,7 +193,7 @@ def get_lib():
     lib.ide3d_raster.argtypes = [C.POINTER(RasterParams), vp]
     lib.ide3d_video_frames.argtypes = [C.POINTER(FramesParams), vp]
     lib.ide3d_image_strips.argtypes = [C.POINTER(StripsParams), vp]
-    for name in ('bias_act', 'upfirdn2d', 'filtered_lrelu', 'filtered_lrelu_act', 'raymarch_fwd', 'raymarch_bwd', 'sample_voxel',
+    for name in ('bias_act', 'upfirdn2d', 'filtered_lrelu', 'filtered_lrelu_act', 'raymarch_fwd', 'raymarch_bwd', 'raymarch_bwd_cam', 'sample_voxel',
                  'sigma_grid', 'planes_to_nhwc', 'initial_rays', 'transform_points', 'sample_triplane', 'integrate',
                  'sample_pdf', 'style_plan', 'mc_classify', 'mc_emit', 'mesh_normals', 'raster', 'video_frames', 'image_strips',
                  'abi_version'):
@@ -207,7 +208,7 @@ def exported_symbols():
     """Names declared in include/ide3d_b200.h (used by the CPU test that checks the .so exports them)."""
     return ['ide3d_abi_version', 'ide3d_last_error', 'ide3d_launch_count', 'ide3d_bias_act', 'ide3d_modconv_epilogue',
             'ide3d_upfirdn2d', 'ide3d_upfirdn2d_add', 'ide3d_upfirdn2d_epilogue',
-            'ide3d_filtered_lrelu', 'ide3d_filtered_lrelu_act', 'ide3d_raymarch_fwd', 'ide3d_raymarch_bwd', 'ide3d_sample_voxel',
+            'ide3d_filtered_lrelu', 'ide3d_filtered_lrelu_act', 'ide3d_raymarch_fwd', 'ide3d_raymarch_bwd', 'ide3d_raymarch_bwd_cam', 'ide3d_sample_voxel',
             'ide3d_sigma_grid', 'ide3d_planes_to_nhwc', 'ide3d_initial_rays', 'ide3d_transform_points',
             'ide3d_sample_triplane', 'ide3d_integrate', 'ide3d_sample_pdf', 'ide3d_mask2color', 'ide3d_style_plan', 'ide3d_mc_classify', 'ide3d_mc_emit',
             'ide3d_mesh_normals', 'ide3d_raster_scratch_bytes', 'ide3d_raster', 'ide3d_video_frames', 'ide3d_image_strips']

@@ -15,8 +15,13 @@
 //           8-lanes-per-texel mapping as the forward gather;  dW1 += da (x) f  per 8-unit block through shared memory (the only true
 //           per-sample outer product),  dW2 / db2 from per-ray sums  sum_s w'_s h_s  (rank-1 again),  db1 += da.
 // Parameter gradients accumulate in a per-CTA shared-memory image of the decoder and are flushed with one atomicAdd per parameter per CTA.
-// Scope: channels-last fp32 planes, the three-head decoder (texture -> 32, shape -> 19, shape -> 1; 64 hidden each).  Camera and
-// per-sample-weight gradients, other decoders and NCHW planes keep the composed-chain path of render_grad.py.
+// Camera gradient (kCam): a sample's grid point is c = b (M[:3,:3] p_cam + M[:3,3]) with p_cam = d_cam z, and neither z nor the
+// compositing deltas depend on M, so  dL/dM[i][j] = b sum_s g_c[i] p_cam[j] (j < 3),  dL/dM[i][3] = b sum_s g_c[i].  g_c, the gradient
+// w.r.t. the grid point, is grid_sampler_2d's grid gradient dotted with df: the scatter reads the plane value at every tap it visits.
+// The 12 sums live in the sample's lane, are reduced per ray into shared memory per CTA and flushed to grad_cam2world[frame] when the
+// CTA moves on to another frame's tiles (12 atomicAdds per frame per CTA, not per ray).
+// Scope: channels-last fp32 planes, the three-head decoder (texture -> 32, shape -> 19, shape -> 1; 64 hidden each).
+// Per-sample-weight gradients, other decoders and NCHW planes keep the composed-chain path of render_grad.py.
 #include "raymarch_common.cuh"
 
 namespace ide3d {
@@ -47,38 +52,71 @@ struct BwdArgs {
     float* g_seg;
     float* g_param[3][4];       // per head: dW1, db1, dW2, db2 (dense, head shapes), or all null
     int tiles_x, tiles_y;
+    float* g_cam;               // [N, 16] zero-initialised (rows 0..2 receive the gradient), or null
 };
 
 using T3 = DecoderTraits<kThreeHead64>;
 
 __device__ __forceinline__ float sigmoid_from_softplus(float h) { return 1.f - __expf(-h); }   // sigmoid(a) = 1 - exp(-softplus(a))
 
-// scatter 4 channel-quads of df (one sample per 8 lanes) into one tri-plane gradient, mirroring gather_chunk_to's taps
+// scatter 4 channel-quads of df (one sample per 8 lanes) into one tri-plane gradient, mirroring gather_chunk_to's taps.
+// kCam: also add to gc[0..2] the gradient of this lane's own sample w.r.t. its grid point (cx, cy, cz) -- grid_sampler_2d's grid
+// gradient (align_corners=False, zeros padding) from the plane values at the same taps, dotted with df.  gbase may then be null
+// (camera-only request: the taps are read, nothing is scattered).
+template <bool kCam = false>
 __device__ __forceinline__ void scatter_chunk(const PlaneView& pv, float* __restrict__ gbase, int n, float cx, float cy, float cz,
-                                              const float* __restrict__ stage, int col0, int lane) {
+                                              const float* __restrict__ stage, int col0, int lane, float (&gc)[3]) {
     const int W = pv.w, H = pv.h;
     const Foot f0 = footprint(cx, cy, W, H), f1 = footprint(cy, cz, W, H), f2 = footprint(cx, cz, W, H);
     const int q = lane & 7, grp = lane >> 3;
     float* base = gbase + (long long)n * pv.sn;
+    const float* pbase = pv.base + (long long)n * pv.sn;
+    const float hw = 0.5f * (float)W, hh = 0.5f * (float)H;                 // d ix / d u, d iy / d v
 #pragma unroll 1
     for (int it = 0; it < 8; ++it) {
         const int src = it * 4 + grp;
         const float4 g = *reinterpret_cast<const float4*>(stage + src * kRow + col0 + q * 4);
+        float gx = 0.f, gy = 0.f, gz = 0.f;                                 // sample src, this lane's 4 channels (kCam)
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
             const Foot& mine = (k == 0) ? f0 : (k == 1 ? f1 : f2);
             const int x0 = __shfl_sync(kFull, mine.x0, src), y0 = __shfl_sync(kFull, mine.y0, src);
             const float fx = __shfl_sync(kFull, mine.fx, src), fy = __shfl_sync(kFull, mine.fy, src);
+            float gu = 0.f, gv = 0.f;
 #pragma unroll
             for (int tap = 0; tap < 4; ++tap) {
                 const int xx = x0 + (tap & 1), yy = y0 + (tap >> 1);
                 const bool ok = ((unsigned)xx < (unsigned)W) && ((unsigned)yy < (unsigned)H);
                 const float wgt = ((tap & 1) ? fx : 1.f - fx) * ((tap >> 1) ? fy : 1.f - fy);
                 if (ok) {
-                    float4* p = reinterpret_cast<float4*>(base + (long long)yy * pv.sh + (long long)xx * pv.sw + k * kFeat + q * 4);
-                    atomicAdd(p, make_float4(g.x * wgt, g.y * wgt, g.z * wgt, g.w * wgt));
+                    if (!kCam || gbase != nullptr) {
+                        float4* p = reinterpret_cast<float4*>(base + (long long)yy * pv.sh + (long long)xx * pv.sw + k * kFeat + q * 4);
+                        atomicAdd(p, make_float4(g.x * wgt, g.y * wgt, g.z * wgt, g.w * wgt));
+                    }
+                    if (kCam) {
+                        // d bil / d ix = sum_taps (+-1) wy P,  d bil / d iy = sum_taps wx (+-1) P
+                        const float4 v = __ldg(reinterpret_cast<const float4*>(pbase + (long long)yy * pv.sh + (long long)xx * pv.sw + k * kFeat + q * 4));
+                        const float dot = v.x * g.x + v.y * g.y + v.z * g.z + v.w * g.w;
+                        const float wy = (tap >> 1) ? fy : 1.f - fy, wx = (tap & 1) ? fx : 1.f - fx;
+                        gu += ((tap & 1) ? wy : -wy) * dot;
+                        gv += ((tap >> 1) ? wx : -wx) * dot;
+                    }
                 }
             }
+            // plane 0 samples (x, y), plane 1 (y, z), plane 2 (x, z)
+            if (k == 0) { gx += hw * gu; gy += hh * gv; }
+            else if (k == 1) { gy += hw * gu; gz += hh * gv; }
+            else { gx += hw * gu; gz += hh * gv; }
+        }
+        if (kCam) {
+            // sum over the 8 lanes of the texel, then hand the total to the lane that owns sample src (= it * 4 + grp)
+#pragma unroll
+            for (int d = 1; d < 8; d <<= 1) {
+                gx += __shfl_xor_sync(kFull, gx, d); gy += __shfl_xor_sync(kFull, gy, d); gz += __shfl_xor_sync(kFull, gz, d);
+            }
+            const int from = (lane & 3) * 8;
+            const float ox = __shfl_sync(kFull, gx, from), oy = __shfl_sync(kFull, gy, from), oz = __shfl_sync(kFull, gz, from);
+            if ((lane >> 2) == it) { gc[0] += ox; gc[1] += oy; gc[2] += oz; }
         }
     }
 }
@@ -101,7 +139,7 @@ __device__ __forceinline__ void hidden8(const float* __restrict__ w1, const floa
     for (int jj = 0; jj < 8; ++jj) h[jj] = softplus_fast(h[jj]);
 }
 
-template <bool kParams>
+template <bool kParams, bool kCam>
 __global__ void __launch_bounds__(kBBlock, 1) raymarch_bwd_kernel(const BwdArgs a) {
     extern __shared__ __align__(16) float smem[];
     float* wsm = smem;                                                      // decoder image (HeadLayout x 3)
@@ -114,9 +152,21 @@ __global__ void __launch_bounds__(kBBlock, 1) raymarch_bwd_kernel(const BwdArgs 
     float* gh = da8 + 32 * 9;                                               // [128] W2^T g of the colour / semantic heads
     float* s_al = gh + 128;                                                 // per-sample: alpha, T, w, q, fac
     float* s_T = s_al + kMaxSteps; float* s_w = s_T + kMaxSteps; float* s_q = s_w + kMaxSteps; float* s_fac = s_q + kMaxSteps;
+    float* cam_sm = per_warp + kBWarps * kPerWarp;                          // kCam: rows 0..2 of dL/dM of frame cam_frame, before * b
     load_decoder<kThreeHead64>(a.dec, wsm);
     if (kParams) for (int i = threadIdx.x; i < T3::kFloats; i += kBBlock) gacc[i] = 0.f;
+    if (kCam && threadIdx.x < 12) cam_sm[threadIdx.x] = 0.f;
     __syncthreads();
+    int cam_frame = -1;
+    // all threads: add the CTA's camera sums of frame `frame` (if any) to the global gradient and clear them
+    auto flush_cam = [&](int frame) {
+        __syncthreads();
+        if (frame >= 0 && threadIdx.x < 12) {
+            atomicAdd(a.g_cam + (long long)frame * 16 + threadIdx.x, a.box_scale * cam_sm[threadIdx.x]);
+            cam_sm[threadIdx.x] = 0.f;
+        }
+        __syncthreads();
+    };
     using L0 = HeadLayout<32, 64, 32>; using L1 = HeadLayout<32, 64, 19>; using L2 = HeadLayout<32, 64, 1>;
     const float* w0 = wsm; const float* w1h = wsm + T3::kOff1; const float* w2h = wsm + T3::kOff2;
 
@@ -127,6 +177,7 @@ __global__ void __launch_bounds__(kBBlock, 1) raymarch_bwd_kernel(const BwdArgs 
 
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int n = tile / tiles_per_frame;
+        if (kCam && n != cam_frame) { flush_cam(cam_frame); cam_frame = n; }      // CTA-uniform: every warp visits every tile
         const int set = plane_set(n, a.views);
         const int t = tile - n * tiles_per_frame;
         const int px = (t % a.tiles_x) * kBTileX + (warp % kBTileX);
@@ -167,7 +218,8 @@ __global__ void __launch_bounds__(kBBlock, 1) raymarch_bwd_kernel(const BwdArgs 
         }
         const float gb = warp_sum(g_lo * w0[L0::kB2 + lane] + ((lane < 19) ? g_hi * w1h[L1::kB2 + lane] : 0.f));
 
-        auto position = [&](int s, bool live, float& zj, float& z1, float& cx, float& cy, float& cz) {
+        // pc: the camera-space point p_cam whose transform gives (cx, cy, cz) / box_scale
+        auto position = [&](int s, bool live, float& zj, float& z1, float& cx, float& cy, float& cz, float (&pc)[3]) {
             float z0 = 0.f, off0 = 0.f;
             z1 = 0.f;
             if (live) {
@@ -190,6 +242,7 @@ __global__ void __launch_bounds__(kBBlock, 1) raymarch_bwd_kernel(const BwdArgs 
             cx = (M[0] * pcx + M[1] * pcy + M[2] * pcz + M[3]) * a.box_scale;
             cy = (M[4] * pcx + M[5] * pcy + M[6] * pcz + M[7]) * a.box_scale;
             cz = (M[8] * pcx + M[9] * pcy + M[10] * pcz + M[11]) * a.box_scale;
+            pc[0] = pcx; pc[1] = pcy; pc[2] = pcz;
             if (!live) { cx = cy = cz = 4.f; }
         };
 
@@ -198,8 +251,8 @@ __global__ void __launch_bounds__(kBBlock, 1) raymarch_bwd_kernel(const BwdArgs 
         for (int ch = 0; ch < chunks; ++ch) {
             const int s = ch * 32 + lane;
             const bool live = s < S;
-            float zj, z1, cx, cy, cz;
-            position(s, live, zj, z1, cx, cy, cz);
+            float zj, z1, cx, cy, cz, pc[3];
+            position(s, live, zj, z1, cx, cy, cz, pc);
             gather_chunk<true>(a.tex, a.seg, set, cx, cy, cz, stage, lane);
             const float* row = stage + lane * kRow;
             float q = gb + gd * zj, sigma = w2h[L2::kB2];
@@ -280,11 +333,14 @@ __global__ void __launch_bounds__(kBBlock, 1) raymarch_bwd_kernel(const BwdArgs 
         // ------------------------------------------------------------------ pass 2: decoder adjoint + scatter
         float hsum[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};                      // sum_s coef_s h_s[j] for j = lane + 32 m  (m: 0,1 colour; 2,3 semantic; 4,5 sigma)
         float wp_sum = 0.f, ds_sum = 0.f;
+        float cam_acc[12];                                                    // kCam: sum_s g_c[i] p_cam[j] at 4 i + j, sum_s g_c[i] at 4 i + 3
+#pragma unroll
+        for (int i = 0; i < 12; ++i) cam_acc[i] = 0.f;
         for (int ch = 0; ch < chunks; ++ch) {
             const int s = ch * 32 + lane;
             const bool live = s < S;
-            float zj, z1, cx, cy, cz;
-            position(s, live, zj, z1, cx, cy, cz);
+            float zj, z1, cx, cy, cz, pc[3];
+            position(s, live, zj, z1, cx, cy, cz, pc);
             gather_chunk<true>(a.tex, a.seg, set, cx, cy, cz, stage, lane);
             float* row = stage + lane * kRow;
             const float wp = live ? s_w[s] : 0.f, ds = live ? s_q[s] : 0.f;
@@ -364,9 +420,28 @@ __global__ void __launch_bounds__(kBBlock, 1) raymarch_bwd_kernel(const BwdArgs 
                 *reinterpret_cast<float4*>(row + kFeat + k) = make_float4(df[k], df[k + 1], df[k + 2], df[k + 3]);
             }
             __syncwarp();
-            if (a.g_tex != nullptr) scatter_chunk(a.tex, a.g_tex, set, cx, cy, cz, stage, 0, lane);
-            if (a.g_seg != nullptr) scatter_chunk(a.seg, a.g_seg, set, cx, cy, cz, stage, kFeat, lane);
+            float gc[3] = {0.f, 0.f, 0.f};
+            if (kCam) {
+                scatter_chunk<true>(a.tex, a.g_tex, set, cx, cy, cz, stage, 0, lane, gc);
+                scatter_chunk<true>(a.seg, a.g_seg, set, cx, cy, cz, stage, kFeat, lane, gc);
+#pragma unroll
+                for (int i = 0; i < 3; ++i) {
+#pragma unroll
+                    for (int j = 0; j < 3; ++j) cam_acc[4 * i + j] = fmaf(gc[i], pc[j], cam_acc[4 * i + j]);
+                    cam_acc[4 * i + 3] += gc[i];
+                }
+            } else {
+                if (a.g_tex != nullptr) scatter_chunk(a.tex, a.g_tex, set, cx, cy, cz, stage, 0, lane, gc);
+                if (a.g_seg != nullptr) scatter_chunk(a.seg, a.g_seg, set, cx, cy, cz, stage, kFeat, lane, gc);
+            }
             __syncwarp();
+        }
+        if (kCam) {
+#pragma unroll
+            for (int i = 0; i < 12; ++i) {
+                const float v = warp_sum(cam_acc[i]);
+                if (lane == 0) atomicAdd(cam_sm + i, v);
+            }
         }
         if (kParams) {
             // rank-1 layer-2 gradients of this ray:  dW2[o][j] += g_o * sum_s w'_s h_s[j];  db2[o] += g_o * sum_s w'_s;  sigma head: coefficient dsigma_s
@@ -386,6 +461,7 @@ __global__ void __launch_bounds__(kBBlock, 1) raymarch_bwd_kernel(const BwdArgs 
         }
     }
 
+    if (kCam) flush_cam(cam_frame);
     if (kParams) {
         __syncthreads();
         // flush the CTA's gradient image: head h, tensor t (W1, b1, W2, b2) -> dense global gradient
@@ -405,8 +481,15 @@ __global__ void __launch_bounds__(kBBlock, 1) raymarch_bwd_kernel(const BwdArgs 
 
 using namespace ide3d;
 
-extern "C" int ide3d_raymarch_bwd(const ide3d_raymarch_params* p, const float* grad_feat, const float* grad_depth, float* grad_tex,
-                                  float* grad_seg, float* const* grad_params, ide3d_stream_t stream) {
+template <bool kParams, bool kCam>
+static int launch_bwd(const BwdArgs& a, int grid, size_t smem, cudaStream_t st) {
+    IDE3D_CUDA(cudaFuncSetAttribute(raymarch_bwd_kernel<kParams, kCam>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    raymarch_bwd_kernel<kParams, kCam><<<grid, kBBlock, smem, st>>>(a);
+    return IDE3D_OK;
+}
+
+static int raymarch_bwd(const ide3d_raymarch_params* p, const float* grad_feat, const float* grad_depth, float* grad_tex,
+                        float* grad_seg, float* const* grad_params, float* grad_cam2world, ide3d_stream_t stream) {
     int rc;
     if ((rc = check_raymarch_params(p)) != IDE3D_OK) return rc;
     IDE3D_REQUIRE(grad_feat != nullptr, "raymarch_bwd: null argument");
@@ -424,19 +507,27 @@ extern "C" int ide3d_raymarch_bwd(const ide3d_raymarch_params* p, const float* g
             IDE3D_REQUIRE(!params || a.g_param[h][t] != nullptr, "raymarch_bwd: parameter gradient %d of head %d missing", t, h);
         }
     a.tiles_x = ceil_div(p->res_w, kBTileX); a.tiles_y = ceil_div(p->res_h, kBTileY);
+    a.g_cam = grad_cam2world;
+    const bool cam = grad_cam2world != nullptr;
     constexpr int kPerWarp = 32 * kRow + 32 * 9 + 128 + 5 * kMaxSteps;
-    const size_t smem = (size_t)(T3::kFloats * (params ? 2 : 1) + kBWarps * kPerWarp) * sizeof(float);
+    const size_t smem = (size_t)(T3::kFloats * (params ? 2 : 1) + kBWarps * kPerWarp + (cam ? 16 : 0)) * sizeof(float);
     const int num_tiles = a.tiles_x * a.tiles_y * a.n;
     int grid = sm_count();
     if (grid > num_tiles) grid = num_tiles;
     cudaStream_t st = (cudaStream_t)stream;
-    if (params) {
-        IDE3D_CUDA(cudaFuncSetAttribute(raymarch_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        raymarch_bwd_kernel<true><<<grid, kBBlock, smem, st>>>(a);
-    } else {
-        IDE3D_CUDA(cudaFuncSetAttribute(raymarch_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        raymarch_bwd_kernel<false><<<grid, kBBlock, smem, st>>>(a);
-    }
+    if (params) rc = cam ? launch_bwd<true, true>(a, grid, smem, st) : launch_bwd<true, false>(a, grid, smem, st);
+    else rc = cam ? launch_bwd<false, true>(a, grid, smem, st) : launch_bwd<false, false>(a, grid, smem, st);
+    if (rc != IDE3D_OK) return rc;
     IDE3D_CHECK_LAUNCH("raymarch_bwd_kernel");
     return IDE3D_OK;
+}
+
+extern "C" int ide3d_raymarch_bwd(const ide3d_raymarch_params* p, const float* grad_feat, const float* grad_depth, float* grad_tex,
+                                  float* grad_seg, float* const* grad_params, ide3d_stream_t stream) {
+    return raymarch_bwd(p, grad_feat, grad_depth, grad_tex, grad_seg, grad_params, nullptr, stream);
+}
+
+extern "C" int ide3d_raymarch_bwd_cam(const ide3d_raymarch_params* p, const float* grad_feat, const float* grad_depth, float* grad_tex,
+                                      float* grad_seg, float* const* grad_params, float* grad_cam2world, ide3d_stream_t stream) {
+    return raymarch_bwd(p, grad_feat, grad_depth, grad_tex, grad_seg, grad_params, grad_cam2world, stream);
 }

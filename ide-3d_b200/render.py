@@ -91,7 +91,8 @@ def raymarch(planes_tex, planes_seg, decoder, cam2world, resolution=(64, 64), nu
     its planes); cam2world and the per-sample tensors have N rows.
     jitter_u: explicit uniforms [N,R,S]; jitter_seed: in-kernel counter hash, one int for the launch, or a sequence / 1-D integer
     tensor of N per-frame seeds (frame f then jitters exactly as a one-frame launch with seed jitter_seed[f]); neither: no jitter.
-    z_vals: explicit sample depths [N,R,S] ascending along S (replaces linspace + jitter; num_steps is taken from it).
+    z_vals: explicit sample depths [N,R,S] ascending along S (replaces linspace + jitter; num_steps is taken from it).  The depths
+    take no gradient (they must not require one); the planes, the camera and the decoder still do.
     precision: 'auto' | 'fp32' (CUDA-core FFMA decoder) | 'tc' (wgmma tensor-core decoder, bf16x3 products).
     Differentiable w.r.t. the planes, the camera and the decoder parameters (when `decoder` is a list of heads holding the
     live parameters): the forward is the same fused kernel, the backward is render_grad.RaymarchFunction."""
@@ -104,8 +105,6 @@ def raymarch(planes_tex, planes_seg, decoder, cam2world, resolution=(64, 64), nu
             raise RuntimeError('ide3d_b200.render.raymarch: z_vals is not differentiable (the reference detaches the importance samples too)')
         kw.update(z_vals=z_vals, num_steps=int(z_vals.shape[-1]))
         num_steps = int(z_vals.shape[-1])
-        if torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in [planes_tex, planes_seg, cam2world]):
-            raise NotImplementedError('ide3d_b200.render.raymarch: the backward pass has no explicit-depth (hierarchical) mode yet')
     if isinstance(decoder, PackedDecoder):
         meta, params = decoder.meta, list(decoder.tensors)
     else:
@@ -124,7 +123,8 @@ def raymarch(planes_tex, planes_seg, decoder, cam2world, resolution=(64, 64), nu
             return _raymarch_impl(tex, seg, heads, cam, jitter_u=ju, noise=nz, **kw)
 
         n = planes_tex.shape[0] * max(int(views), 1)
-        feat, depth, weights = render_grad.RaymarchFunction.apply(fwd, cfg, meta, jitter_u, noise, bool(return_weights), planes_tex.float(),
+        zv = None if z_vals is None else z_vals.detach()
+        feat, depth, weights = render_grad.RaymarchFunction.apply(fwd, cfg, meta, jitter_u, noise, zv, bool(return_weights), planes_tex.float(),
                                                                   planes_seg.float(), cam2world.reshape(n, 4, 4).float(), *params)
         return feat, depth, (weights if return_weights else None)
     return _raymarch_impl(planes_tex, planes_seg, decoder, cam2world, jitter_u=jitter_u, noise=noise, **kw)
@@ -150,7 +150,6 @@ def coarse_depths(n, resolution, num_steps, ray_start=2.25, ray_end=3.3, jitter_
     return zv + (jitter_u.to(device=device, dtype=torch.float32).reshape(n, R, S) - 0.5) * spacing
 
 
-@torch.no_grad()
 def raymarch_hierarchical(planes_tex, planes_seg, decoder, cam2world, resolution=(64, 64), num_steps=48, n_importance=None,
                           ray_start=2.25, ray_end=3.3, jitter_u=None, jitter_seed=None, importance_u=None, det=False,
                           return_weights=False, return_depths=False, views=1, **kw):
@@ -162,7 +161,9 @@ def raymarch_hierarchical(planes_tex, planes_seg, decoder, cam2world, resolution
         3. the coarse and fine depths merged and sorted per ray; second fused pass over all S + n_importance samples with the depths
            read from that tensor (IDE3D_JITTER_ZVALS) -- compositing over the merged set, as the reference composition does.
     views, jitter_seed: as in `raymarch` (N = planes * views frames).
-    Forward only.  -> feat [N,R,51], depth [N,R,1], weights [N,R,S+n_importance,1] | None (, z_vals [N,R,S+n_importance])."""
+    Differentiable like `raymarch` w.r.t. the planes, the camera and the decoder (a list of heads holding the live parameters) through
+    the second pass; the coarse pass and the importance depths are detached, as in pi-GAN / StyleNeRF.
+    -> feat [N,R,51], depth [N,R,1], weights [N,R,S+n_importance,1] | None (, z_vals [N,R,S+n_importance])."""
     from .training.volumetric_rendering import sample_pdf_u
     L.require_cuda(planes_tex, planes_seg, cam2world)
     dev = planes_tex.device
@@ -171,26 +172,32 @@ def raymarch_hierarchical(planes_tex, planes_seg, decoder, cam2world, resolution
     R, S = W * H, int(num_steps)
     n_imp = S if n_importance is None else int(n_importance)
     assert S >= 3, 'hierarchical sampling needs at least 3 coarse samples (weights[1:-1])'
-    tex, seg = as_planes(planes_tex), as_planes(planes_seg)
-    dec = _decoder(decoder, dev)
-    z = coarse_depths(n, (W, H), S, ray_start, ray_end, jitter_u=jitter_u, jitter_seed=jitter_seed, device=dev)
-    kw = dict(kw, convert_layout=False, views=views)
+    params = [] if isinstance(decoder, PackedDecoder) else [t for h in decoder for t in h[2:6]]
+    grad = torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in [planes_tex, planes_seg, cam2world] + params)
+    kw = dict(kw, views=views)
+    kw.pop('convert_layout', None)
     noise_std = float(kw.pop('noise_std', 0.0) or 0.0)
     kw.pop('noise', None)                                  # drawn per pass (the two passes have different sample counts)
     draw = (lambda s_: dict(noise=torch.randn(n, R, s_, device=dev), noise_std=noise_std)) if noise_std else (lambda s_: {})
-    _, _, w = _raymarch_impl(tex, seg, dec, cam2world, resolution=(W, H), ray_start=ray_start, ray_end=ray_end, z_vals=z,
-                             num_steps=S, return_weights=True, **draw(S), **kw)
-    z_mid = 0.5 * (z[..., :-1] + z[..., 1:])
-    if det:
-        u = torch.linspace(0, 1, n_imp, device=dev).expand(n * R, n_imp)
-    elif importance_u is not None:
-        u = importance_u.to(device=dev, dtype=torch.float32).reshape(n * R, n_imp)
-    else:
-        u = torch.rand(n * R, n_imp, device=dev)
-    fine = sample_pdf_u(z_mid.reshape(n * R, S - 1), w.reshape(n * R, S)[:, 1:-1] + 1e-5, u)
-    all_z = torch.sort(torch.cat([z, fine.reshape(n, R, n_imp)], -1), dim=-1).values
-    feat, depth, weights = _raymarch_impl(tex, seg, dec, cam2world, resolution=(W, H), ray_start=ray_start, ray_end=ray_end,
-                                          z_vals=all_z, num_steps=S + n_imp, return_weights=return_weights, **draw(S + n_imp), **kw)
+    with torch.no_grad():
+        tex, seg = as_planes(planes_tex), as_planes(planes_seg)
+        dec = _decoder(decoder, dev)
+        z = coarse_depths(n, (W, H), S, ray_start, ray_end, jitter_u=jitter_u, jitter_seed=jitter_seed, device=dev)
+        _, _, w = _raymarch_impl(tex, seg, dec, cam2world, resolution=(W, H), ray_start=ray_start, ray_end=ray_end, z_vals=z,
+                                 num_steps=S, return_weights=True, convert_layout=False, **draw(S), **kw)
+        z_mid = 0.5 * (z[..., :-1] + z[..., 1:])
+        if det:
+            u = torch.linspace(0, 1, n_imp, device=dev).expand(n * R, n_imp)
+        elif importance_u is not None:
+            u = importance_u.to(device=dev, dtype=torch.float32).reshape(n * R, n_imp)
+        else:
+            u = torch.rand(n * R, n_imp, device=dev)
+        fine = sample_pdf_u(z_mid.reshape(n * R, S - 1), w.reshape(n * R, S)[:, 1:-1] + 1e-5, u)
+        all_z = torch.sort(torch.cat([z, fine.reshape(n, R, n_imp)], -1), dim=-1).values
+    # second pass: under grad the caller's tensors (autograd sees the layout conversion and the live heads), else the converted ones
+    src = (planes_tex, planes_seg, decoder) if grad else (tex, seg, dec)
+    feat, depth, weights = raymarch(*src, cam2world, resolution=(W, H), ray_start=ray_start, ray_end=ray_end, z_vals=all_z,
+                                    return_weights=return_weights, convert_layout=grad, **draw(S + n_imp), **kw)
     return (feat, depth, weights, all_z) if return_depths else (feat, depth, weights)
 
 
@@ -311,10 +318,12 @@ def sigma_grid(planes_tex, planes_seg, decoder, grid_n=256, voxel_origin=(0, 0, 
 def raymarch_backward(planes_tex, planes_seg, decoder, cam2world, grad_feat, grad_depth, resolution=(64, 64), num_steps=48, fov=18.0,
                       ray_start=2.25, ray_end=3.3, box_scale=2.0, jitter_u=None, jitter_seed=None, noise=None, noise_std=0.0,
                       clamp_mode='softplus', last_back=False, white_back=False, max_depth=None, fill_mode=None, z_vals=None,
-                      want_planes=(True, True), want_params=True, views=1):
+                      want_planes=(True, True), want_params=True, views=1, want_camera=False):
     """ide3d_raymarch_bwd: gradients of (feat, depth) of `raymarch` w.r.t. the planes and the three decoder heads, one kernel that
     recomputes the per-sample chain (no materialised intermediates).  -> (d_tex | None, d_seg | None, [dW1, db1, dW2, db2] x 3 | None),
     or None when the configuration has no backward kernel (the caller then differentiates the composed chain).
+    want_camera: ide3d_raymarch_bwd_cam, which also returns d_cam [N,4,4] (row 3 zero) as a fourth element.  The sample depths
+    (jitter, z_vals) take no gradient.
     views: as in `raymarch`; the plane gradients of all views of a plane set accumulate into that set's gradient."""
     p, tex, seg, dec, keep = _raymarch_params(planes_tex, planes_seg, decoder, cam2world, resolution, num_steps, fov, ray_start, ray_end,
                                               box_scale, jitter_u, jitter_seed, noise, noise_std, clamp_mode, last_back, white_back,
@@ -335,8 +344,13 @@ def raymarch_backward(planes_tex, planes_seg, decoder, cam2world, grad_feat, gra
     ptrs = None
     if d_par is not None:
         ptrs = (C.c_void_p * 12)(*[t.data_ptr() for t in d_par])
+    d_cam = torch.zeros(n, 16, dtype=torch.float32, device=dev) if want_camera else None
     with torch.cuda.device(dev):
-        rc = L.get_lib().ide3d_raymarch_bwd(C.byref(p), L.ptr(gf), L.ptr(gd), L.ptr(d_tex), L.ptr(d_seg), ptrs, L.stream_ptr(dev))
+        if want_camera:
+            rc = L.get_lib().ide3d_raymarch_bwd_cam(C.byref(p), L.ptr(gf), L.ptr(gd), L.ptr(d_tex), L.ptr(d_seg), ptrs, L.ptr(d_cam),
+                                                    L.stream_ptr(dev))
+        else:
+            rc = L.get_lib().ide3d_raymarch_bwd(C.byref(p), L.ptr(gf), L.ptr(gd), L.ptr(d_tex), L.ptr(d_seg), ptrs, L.stream_ptr(dev))
     if L.check(rc, allow_unsupported=True) == L.UNSUPPORTED:
         return None
-    return d_tex, d_seg, d_par
+    return (d_tex, d_seg, d_par, d_cam.reshape(n, 4, 4)) if want_camera else (d_tex, d_seg, d_par)

@@ -16,7 +16,7 @@ import torch
 import torch.nn.functional as F
 
 N_FEAT, N_OUT = 32, 52
-USE_BACKWARD_KERNEL = True    # ide3d_raymarch_bwd for the planes / decoder gradients; False = always differentiate the composed chain
+USE_BACKWARD_KERNEL = True    # ide3d_raymarch_bwd(_cam) for the planes / decoder / camera gradients; False = always differentiate the composed chain
 RAYS_PER_SLAB = 1024          # rays per recompute slab: bounds the materialised [n, rays, S, 52+64+...] tensors
 
 
@@ -64,11 +64,12 @@ def _decode(f_tex, f_seg, heads):
     return out
 
 
-def composed_chain(tex, seg, heads, cam2world, cfg, jitter_u=None, noise=None, rays=None):
+def composed_chain(tex, seg, heads, cam2world, cfg, jitter_u=None, noise=None, rays=None, z_vals=None):
     """The renderer chain on materialised tensors.  tex/seg [n,96,H,W]; cam2world [n,4,4]; cfg: dict(W, H, S, fov, ray_start,
     ray_end, box_scale, jitter_seed, noise_std, clamp_mode, last_back, white_back, max_depth, fill_weight[, views]).
     views > 1: the planes hold n / views sets, frame f reads set f // views (materialised here by repeat_interleave, so autograd sums
     the views' gradients into their set); jitter_seed may be a list of per-frame seeds.
+    z_vals: explicit sample depths [n,R,S] (render.raymarch's z_vals), used in place of linspace + jitter; they take no gradient.
     rays: optional (first, count) slab of the R = W*H rays.  -> feat [n,r,51], depth [n,r,1], weights [n,r,S,1]."""
     views = int(cfg.get('views', 1) or 1)
     if views > 1:
@@ -86,17 +87,20 @@ def composed_chain(tex, seg, heads, cam2world, cfg, jitter_u=None, noise=None, r
     d = torch.stack([x, y, z], -1)
     d = d / d.norm(dim=-1, keepdim=True)                                     # [r,3]
     zv = torch.linspace(cfg['ray_start'], cfg['ray_end'], S, device=dev)
-    z_vals = zv.reshape(1, 1, S).expand(n, rc, S)
     u = None
-    if jitter_u is not None:
-        u = jitter_u.reshape(n, R, S)[:, r0:r0 + rc]
-    elif cfg.get('jitter_seed') is not None:
-        from .render import frame_seeds
-        seeds = frame_seeds(cfg['jitter_seed'])
-        if seeds is None:
-            u = torch.stack([hash_uniform(rc * S, cfg['jitter_seed'], dev, first=(i * R + r0) * S).reshape(rc, S) for i in range(n)])
-        else:
-            u = hash_uniform_frames(rc * S, seeds, dev, first=r0 * S).reshape(n, rc, S)
+    if z_vals is not None:
+        z_vals = z_vals.detach().to(device=dev, dtype=torch.float32).reshape(n, R, S)[:, r0:r0 + rc]
+    else:
+        z_vals = zv.reshape(1, 1, S).expand(n, rc, S)
+        if jitter_u is not None:
+            u = jitter_u.reshape(n, R, S)[:, r0:r0 + rc]
+        elif cfg.get('jitter_seed') is not None:
+            from .render import frame_seeds
+            seeds = frame_seeds(cfg['jitter_seed'])
+            if seeds is None:
+                u = torch.stack([hash_uniform(rc * S, cfg['jitter_seed'], dev, first=(i * R + r0) * S).reshape(rc, S) for i in range(n)])
+            else:
+                u = hash_uniform_frames(rc * S, seeds, dev, first=r0 * S).reshape(n, rc, S)
     if u is not None and S > 1:
         z_vals = z_vals + (u - 0.5) * (zv[1] - zv[0])
     pts = d.reshape(1, rc, 1, 3) * z_vals.unsqueeze(-1)                      # camera space
@@ -133,35 +137,36 @@ class RaymarchFunction(torch.autograd.Function):
     """forward: render._raymarch_fwd (fused kernel).  backward: autograd through `composed_chain`, slab by slab."""
 
     @staticmethod
-    def forward(ctx, fwd, cfg, head_meta, jitter_u, noise, want_weights, tex, seg, cam2world, *params):
+    def forward(ctx, fwd, cfg, head_meta, jitter_u, noise, z_vals, want_weights, tex, seg, cam2world, *params):
         heads = [(m[0], m[1]) + tuple(params[4 * i:4 * i + 4]) for i, m in enumerate(head_meta)]
         feat, depth, weights = fwd(tex, seg, heads, cam2world, jitter_u, noise)
         ctx.cfg, ctx.head_meta, ctx.want_weights = cfg, head_meta, want_weights
-        ctx.save_for_backward(tex, seg, cam2world, jitter_u, noise, *params)
+        ctx.save_for_backward(tex, seg, cam2world, jitter_u, noise, z_vals, *params)
         if weights is None:
             weights = feat.new_zeros(())
         return feat, depth, weights
 
     @staticmethod
     def backward(ctx, dfeat, ddepth, dweights):
-        tex, seg, cam2world, jitter_u, noise, *params = ctx.saved_tensors
+        tex, seg, cam2world, jitter_u, noise, z_vals, *params = ctx.saved_tensors
         cfg = ctx.cfg
-        need = ctx.needs_input_grad[6:]
-        # fast path: the backward kernel (ide3d_raymarch_bwd) -- planes + three-head decoder, no camera / per-sample-weight gradients
+        need = ctx.needs_input_grad[7:]
+        # fast path: the backward kernel (ide3d_raymarch_bwd_cam) -- planes, three-head decoder and camera; no per-sample-weight gradients
         want_w = ctx.want_weights and dweights is not None and dweights.ndim == 4 and bool((dweights != 0).any())
-        if USE_BACKWARD_KERNEL and tex.is_cuda and not need[2] and not want_w:
+        if USE_BACKWARD_KERNEL and tex.is_cuda and not want_w:
             from . import render
             heads = [(m[0], m[1]) + tuple(params[4 * i:4 * i + 4]) for i, m in enumerate(ctx.head_meta)]
             kw = dict(resolution=(cfg['W'], cfg['H']), num_steps=cfg['S'], fov=cfg['fov'], ray_start=cfg['ray_start'], ray_end=cfg['ray_end'],
                       box_scale=cfg['box_scale'], jitter_u=jitter_u, jitter_seed=cfg.get('jitter_seed'), noise=noise, noise_std=cfg.get('noise_std', 0.0),
                       clamp_mode=cfg['clamp_mode'], last_back=cfg['last_back'], white_back=cfg['white_back'], max_depth=cfg['max_depth'],
-                      fill_mode='weight' if cfg['fill_weight'] else None, views=cfg.get('views', 1))
+                      fill_mode='weight' if cfg['fill_weight'] else None, views=cfg.get('views', 1), z_vals=z_vals)
             res = render.raymarch_backward(tex, seg, heads, cam2world, dfeat, ddepth, want_planes=(bool(need[0]), bool(need[1])),
-                                           want_params=any(need[3:]), **kw)
+                                           want_params=any(need[3:]), want_camera=bool(need[2]), **kw)
             if res is not None:
-                d_tex, d_seg, d_par = res
+                d_tex, d_seg, d_par = res[:3]
+                d_cam = res[3].to(cam2world.dtype) if need[2] else None
                 gp = [None] * len(params) if d_par is None else [g.reshape(p.shape).to(p.dtype) if nd else None for g, p, nd in zip(d_par, params, need[3:])]
-                return (None, None, None, None, None, None, d_tex if need[0] else None, d_seg if need[1] else None, None) + tuple(gp)
+                return (None,) * 7 + (d_tex if need[0] else None, d_seg if need[1] else None, d_cam) + tuple(gp)
         leaves = [t.detach().requires_grad_(bool(nd)) for t, nd in zip((tex, seg, cam2world) + tuple(params), need)]
         wanted = [t for t in leaves if t.requires_grad]
         grads = [torch.zeros_like(t) for t in wanted]
@@ -172,7 +177,7 @@ class RaymarchFunction(torch.autograd.Function):
             for r0 in range(0, R, RAYS_PER_SLAB):
                 rc = min(RAYS_PER_SLAB, R - r0)
                 with torch.enable_grad():
-                    feat, depth, weights = composed_chain(l_tex, l_seg, heads, l_cam, cfg, jitter_u, noise, rays=(r0, rc))
+                    feat, depth, weights = composed_chain(l_tex, l_seg, heads, l_cam, cfg, jitter_u, noise, rays=(r0, rc), z_vals=z_vals)
                     outs, gouts = [feat, depth], [dfeat[:, r0:r0 + rc], ddepth[:, r0:r0 + rc]]
                     if ctx.want_weights and dweights is not None and dweights.ndim == 4:
                         outs.append(weights); gouts.append(dweights[:, r0:r0 + rc])
@@ -182,4 +187,4 @@ class RaymarchFunction(torch.autograd.Function):
                         acc.add_(gi)
         it = iter(grads)
         out = [next(it) if t.requires_grad else None for t in leaves]
-        return (None, None, None, None, None, None) + tuple(out)
+        return (None,) * 7 + tuple(out)

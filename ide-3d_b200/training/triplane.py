@@ -108,7 +108,8 @@ class TriPlaneRenderer(torch.nn.Module):
         views: frames per plane set; img_v / seg_v hold N / views sets and cam2world N rows, view j of set i being frame
         i * views + j.  seed: one int, or N per-frame seeds (frame f then jitters as a one-frame call with seed[f]).
         hierarchical: two-pass importance sampling (render.raymarch_hierarchical; sample_pdf, volumetric_rendering.py:224-265) with
-        n_importance (default num_steps) extra samples per ray; forward only.  Off by default: whether the released generator samples
+        n_importance (default num_steps) extra samples per ray; gradients flow through the second pass, the importance depths are
+        detached.  Off by default: whether the released generator samples
         hierarchically is not recoverable from the reference tree (SURVEY.md a8).
         perturb: 'hash' (in-kernel counter hash seeded from torch's CPU generator), 'rand' (torch.rand on the device,
         the draw the reference makes at volumetric_rendering.py:101), or None/False (no jitter)."""
@@ -124,9 +125,7 @@ class TriPlaneRenderer(torch.nn.Module):
         # live parameters (differentiable) when a gradient can reach them, else the cached device copy
         train = torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())
         if hierarchical:
-            if train or (torch.is_grad_enabled() and (img_v.requires_grad or seg_v.requires_grad or cam2world.requires_grad)):
-                raise NotImplementedError('TriPlaneRenderer: hierarchical sampling is forward-only (run under torch.no_grad())')
-            return render.raymarch_hierarchical(img_v, seg_v, self.packed(), cam2world, resolution=res, num_steps=num_steps,
+            return render.raymarch_hierarchical(img_v, seg_v, self.heads() if train else self.packed(), cam2world, resolution=res, num_steps=num_steps,
                                                 n_importance=n_importance, fov=fov, ray_start=ray_start, ray_end=ray_end,
                                                 box_scale=self.box_scale, jitter_u=jitter_u, jitter_seed=seed, importance_u=importance_u,
                                                 det=perturb in (None, False, 'none'), noise_std=float(nerf_noise or 0.0),

@@ -258,6 +258,14 @@ int ide3d_raymarch_fwd(const ide3d_raymarch_params* p, ide3d_stream_t stream);
 int ide3d_raymarch_bwd(const ide3d_raymarch_params* p, const float* grad_feat, const float* grad_depth, float* grad_tex,
                        float* grad_seg, float* const* grad_params, ide3d_stream_t stream);
 
+/* ide3d_raymarch_bwd plus the gradient w.r.t. the camera: grad_cam2world [N,16] fp32 (row-major 4x4 per frame, like cam2world),
+ * ZERO-INITIALISED by the caller and accumulated into; rows 0..2 receive dL/dM, row 3 stays 0.  The sample depths (linspace + jitter,
+ * or the ZVALS tensor) do not depend on the camera.  grad_cam2world == NULL behaves exactly like ide3d_raymarch_bwd, and the other
+ * arguments, the validation and the unsupported configurations are those of ide3d_raymarch_bwd; grad_tex, grad_seg and grad_params may
+ * all be NULL (camera-only refinement). */
+int ide3d_raymarch_bwd_cam(const ide3d_raymarch_params* p, const float* grad_feat, const float* grad_depth, float* grad_tex,
+                           float* grad_seg, float* const* grad_params, float* grad_cam2world, ide3d_stream_t stream);
+
 /* sample_voxel: decode `points` [N, P, 3] (world units) -> out [N, P, 52], or, with sigma_only,
  * out [N, P] holding channel 51 only. */
 int ide3d_sample_voxel(const ide3d_triplane* tex, const ide3d_triplane* seg, const ide3d_decoder* dec,
