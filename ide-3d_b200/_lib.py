@@ -118,6 +118,21 @@ class StripsParams(C.Structure):
                 ('lut', C.c_void_p), ('out_image', C.c_void_p), ('out_seg', C.c_void_p)]
 
 
+NOISE_MAX_BUFFERS = 64                                 # IDE3D_NOISE_MAX_BUFFERS
+
+
+class NoiseTable(C.Structure):
+    _fields_ = [('count', C.c_int), ('sides', C.c_int * NOISE_MAX_BUFFERS), ('bufs', C.c_void_p * NOISE_MAX_BUFFERS),
+                ('grads', C.c_void_p * NOISE_MAX_BUFFERS), ('scratch', C.c_void_p), ('scratch_floats', C.c_int64)]
+
+
+class SegXentParams(C.Structure):
+    _fields_ = [('seg', C.c_void_p), ('n', C.c_int), ('classes', C.c_int), ('in_h', C.c_int), ('in_w', C.c_int),
+                ('seg_stride_n', C.c_int64), ('seg_stride_c', C.c_int64), ('seg_stride_h', C.c_int64), ('seg_stride_w', C.c_int64),
+                ('mask', C.c_void_p), ('out_h', C.c_int), ('out_w', C.c_int), ('lse', C.c_void_p), ('partials', C.c_void_p),
+                ('loss', C.c_void_p), ('grad_loss', C.c_void_p), ('grad_seg', C.c_void_p)]
+
+
 _lib = None
 
 
@@ -193,10 +208,14 @@ def get_lib():
     lib.ide3d_raster.argtypes = [C.POINTER(RasterParams), vp]
     lib.ide3d_video_frames.argtypes = [C.POINTER(FramesParams), vp]
     lib.ide3d_image_strips.argtypes = [C.POINTER(StripsParams), vp]
+    lib.ide3d_noise_reg.argtypes = [C.POINTER(NoiseTable), vp, vp, vp]
+    lib.ide3d_noise_normalize.argtypes = [C.POINTER(NoiseTable), vp]
+    lib.ide3d_seg_xent_fwd.argtypes = [C.POINTER(SegXentParams), vp]
+    lib.ide3d_seg_xent_bwd.argtypes = [C.POINTER(SegXentParams), vp]
     for name in ('bias_act', 'upfirdn2d', 'filtered_lrelu', 'filtered_lrelu_act', 'raymarch_fwd', 'raymarch_bwd', 'raymarch_bwd_cam', 'sample_voxel',
                  'sigma_grid', 'planes_to_nhwc', 'initial_rays', 'transform_points', 'sample_triplane', 'integrate',
                  'sample_pdf', 'style_plan', 'mc_classify', 'mc_emit', 'mesh_normals', 'raster', 'video_frames', 'image_strips',
-                 'abi_version'):
+                 'noise_reg', 'noise_normalize', 'seg_xent_fwd', 'seg_xent_bwd', 'abi_version'):
         getattr(lib, 'ide3d_' + name).restype = C.c_int
     if lib.ide3d_abi_version() != 1:
         raise RuntimeError('ide3d_b200: ABI version mismatch between _lib.py and libide3d_b200.so')
@@ -211,7 +230,8 @@ def exported_symbols():
             'ide3d_filtered_lrelu', 'ide3d_filtered_lrelu_act', 'ide3d_raymarch_fwd', 'ide3d_raymarch_bwd', 'ide3d_raymarch_bwd_cam', 'ide3d_sample_voxel',
             'ide3d_sigma_grid', 'ide3d_planes_to_nhwc', 'ide3d_initial_rays', 'ide3d_transform_points',
             'ide3d_sample_triplane', 'ide3d_integrate', 'ide3d_sample_pdf', 'ide3d_mask2color', 'ide3d_style_plan', 'ide3d_mc_classify', 'ide3d_mc_emit',
-            'ide3d_mesh_normals', 'ide3d_raster_scratch_bytes', 'ide3d_raster', 'ide3d_video_frames', 'ide3d_image_strips']
+            'ide3d_mesh_normals', 'ide3d_raster_scratch_bytes', 'ide3d_raster', 'ide3d_video_frames', 'ide3d_image_strips',
+            'ide3d_noise_reg', 'ide3d_noise_normalize', 'ide3d_seg_xent_fwd', 'ide3d_seg_xent_bwd']
 
 
 def check(rc, allow_unsupported=False):

@@ -45,4 +45,28 @@ __device__ __forceinline__ int seg_class_at(const float* s, int classes, int in_
     return arg;
 }
 
+// The taps of output pixel (x, y) and the logit of one class there, with seg_class_at's arithmetic (projector.cu's cross-entropy
+// evaluates one class at a time from these).
+struct SegTaps {
+    const float *r0, *r1;
+    long long c0, c1;
+    Tap tx, ty;
+};
+__device__ __forceinline__ SegTaps seg_taps_at(const float* s, int in_h, int in_w, long long sh, long long sw, int x, int y, int out_h,
+                                               int out_w) {
+    SegTaps t;
+    t.ty = bilinear_tap(y, in_h, out_h);
+    t.tx = bilinear_tap(x, in_w, out_w);
+    t.r0 = s + t.ty.i0 * sh;
+    t.r1 = s + t.ty.i1 * sh;
+    t.c0 = t.tx.i0 * sw;
+    t.c1 = t.tx.i1 * sw;
+    return t;
+}
+__device__ __forceinline__ float seg_logit_at(const SegTaps& t, long long kc) {
+    const float top = __fadd_rn(__fmul_rn(t.tx.l0, __ldg(t.r0 + kc + t.c0)), __fmul_rn(t.tx.l1, __ldg(t.r0 + kc + t.c1)));
+    const float bot = __fadd_rn(__fmul_rn(t.tx.l0, __ldg(t.r1 + kc + t.c0)), __fmul_rn(t.tx.l1, __ldg(t.r1 + kc + t.c1)));
+    return __fadd_rn(__fmul_rn(t.ty.l0, top), __fmul_rn(t.ty.l1, bot));
+}
+
 }  // namespace ide3d

@@ -227,7 +227,9 @@ class SynthesisLayer(torch.nn.Module):
         noise = None
         if self.use_noise and noise_mode == 'random':
             noise = torch.randn([x.shape[0], 1, self.up * x.shape[2], self.up * x.shape[3]], device=x.device) * self.noise_strength
-        inference = not (torch.is_grad_enabled() and (self.weight.requires_grad or (self.use_noise and self.noise_strength.requires_grad)))
+        # a projector freezes the layer but optimises noise_const (inversion/training/projectors/w_projector_ide3d.py:79-85)
+        inference = not (torch.is_grad_enabled() and (self.weight.requires_grad or (self.use_noise and (
+            self.noise_strength.requires_grad or self.noise_const.requires_grad))))
         if self.use_noise and noise_mode == 'const':
             # constants of the weights, cached per parameter version for inference (one multiply / one 9 MB weight copy per layer and step otherwise)
             noise = self._cached('noise', (self.noise_const, self.noise_strength), lambda: self.noise_const * self.noise_strength) if inference \

@@ -87,6 +87,10 @@ class TriPlaneRenderer(torch.nn.Module):
             self._packed_key = key
         return self._packed
 
+    def __getstate__(self):
+        # the packed decoder holds ctypes structs of device pointers: copies and pickles rebuild it on their first call
+        return dict(super().__getstate__(), _packed=None, _packed_key=None)
+
     as_planes = staticmethod(render.as_planes)
 
     def sample_voxel(self, img_v, seg_v, points, sigma_only=False):

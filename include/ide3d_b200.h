@@ -26,6 +26,9 @@
  *   ide3d_planes_to_nhwc      layout helper for the two kernels above (no reference counterpart).
  *   ide3d_mesh_normals        render_mesh.py:36-42  smooth vertex normals (trimesh / pyrender smooth=True)
  *   ide3d_raster              render_mesh.py:44-61  shaded frames of the mesh (pyrender OffscreenRenderer)
+ *   ide3d_noise_reg           inversion/training/projectors/w_projector_ide3d.py:113-122  noise regulariser (+ its gradient)
+ *   ide3d_noise_normalize     inversion/training/projectors/w_projector_ide3d.py:138-142  noise renormalisation
+ *   ide3d_seg_xent_fwd/_bwd   semantic-mask loss of the projector (extension): cross-entropy of the upsampled logits
  *
  * Conventions
  *   - plain C: raw device pointers, sizes, strides (in ELEMENTS), a cudaStream_t passed as void*.
@@ -444,6 +447,54 @@ typedef struct ide3d_style_layer {
 } ide3d_style_layer;
 int ide3d_style_plan(const float* ws, int n, int num_ws, int w_dim, const ide3d_style_layer* layers, int num_layers,
                      float* styles, float* dcoefs, ide3d_stream_t stream);
+
+/* Noise regulariser of the projectors (inversion/training/projectors/w_projector_ide3d.py:113-122) over a table of `count` noise
+ * buffers, each a dense fp32 [side, side] map (the SynthesisLayer.noise_const buffers).  Per buffer, at pyramid levels L = 0, 1, ...
+ * (level L + 1 = avg_pool2d(level L, 2), stopping after the first level whose side is <= 8):
+ *   reg = sum over buffers and levels of mean(n * roll(n, 1, W))^2 + mean(n * roll(n, 1, H))^2
+ * ide3d_noise_reg writes reg to loss[0] (device).  With grad_scale (device scalar) != NULL it also writes, for every buffer,
+ * grads[b] = grad_scale[0] * d reg / d bufs[b]: the sum over levels of (1/4)^L times the level-L gradient at the pixel's ancestor.
+ * ide3d_noise_normalize renormalises every buffer in place (:138-142): buf -= mean(buf); buf *= rsqrt(mean(buf^2)).
+ * Two launches (noise_reg) and one (noise_normalize), whatever the number of buffers; reductions run in a fixed order (no float
+ * atomics), so two calls give bit-identical results.
+ * scratch: device memory, 8-byte aligned, at least 128 + sum over buffers of sum_{L >= 1} (side >> L)^2 floats (the pyramid levels
+ * above the buffer and one double per buffer); noise_normalize does not use it.
+ * IDE3D_UNSUPPORTED for count > IDE3D_NOISE_MAX_BUFFERS or a side that is not a power of two in [1, 512]. */
+#define IDE3D_NOISE_MAX_BUFFERS 64
+typedef struct ide3d_noise_table {
+    int count;
+    int sides[IDE3D_NOISE_MAX_BUFFERS];
+    float* bufs[IDE3D_NOISE_MAX_BUFFERS];
+    float* grads[IDE3D_NOISE_MAX_BUFFERS];   /* noise_reg with grad_scale only */
+    float* scratch;
+    int64_t scratch_floats;
+} ide3d_noise_table;
+int ide3d_noise_reg(const ide3d_noise_table* t, float* loss, const float* grad_scale, ide3d_stream_t stream);
+int ide3d_noise_normalize(const ide3d_noise_table* t, ide3d_stream_t stream);
+
+/* Semantic-mask loss of the projector (extension): F.cross_entropy(interpolate(seg, (out_h, out_w), 'bilinear', align_corners=False),
+ * mask), mean over the n * out_h * out_w pixels, without building the upsampled logits.  seg [n, classes, in_h, in_w] fp32, any
+ * strides (e.g. the strided view G.synthesis(..., return_seg='raw') returns); mask uint8 [n, out_h, out_w] dense, values < classes.
+ *   ide3d_seg_xent_fwd: per output pixel the bilinear logits (the rounding of ide3d_image_strips), their log-sum-exp -> lse
+ *                       [n, out_h, out_w] (kept for the backward), loss[0] = mean(lse - logit[mask]).  partials: n * out_h doubles.
+ *   ide3d_seg_xent_bwd: grad_seg [n, classes, in_h, in_w] dense = grad_loss[0] * the adjoint of the upsampling applied to
+ *                       (softmax - onehot(mask)) / (n * out_h * out_w); every texel gathers the output pixels whose taps reach it.
+ * No float atomics: both are deterministic.  Limits: classes <= 32; every tensor's element offsets fit 31 bits.
+ * The mask is not validated on the device: a label >= classes is read as classes - 1 (F.cross_entropy would raise); callers check it. */
+typedef struct ide3d_seg_xent_params {
+    const float* seg;
+    int n, classes, in_h, in_w;
+    int64_t seg_stride_n, seg_stride_c, seg_stride_h, seg_stride_w;
+    const uint8_t* mask;
+    int out_h, out_w;
+    float* lse;                 /* [n, out_h, out_w]: written by fwd, read by bwd */
+    double* partials;           /* fwd: [n * out_h] */
+    float* loss;                /* fwd: [1] */
+    const float* grad_loss;     /* bwd: [1] */
+    float* grad_seg;            /* bwd: [n, classes, in_h, in_w] */
+} ide3d_seg_xent_params;
+int ide3d_seg_xent_fwd(const ide3d_seg_xent_params* p, ide3d_stream_t stream);
+int ide3d_seg_xent_bwd(const ide3d_seg_xent_params* p, ide3d_stream_t stream);
 
 #ifdef __cplusplus
 }
