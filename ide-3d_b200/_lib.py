@@ -133,6 +133,20 @@ class SegXentParams(C.Structure):
                 ('loss', C.c_void_p), ('grad_loss', C.c_void_p), ('grad_seg', C.c_void_p)]
 
 
+LPIPS_MAX_LAYERS = 8                                   # IDE3D_LPIPS_MAX_LAYERS
+
+
+class LpipsLayer(C.Structure):
+    _fields_ = [('c', C.c_int), ('h', C.c_int), ('w', C.c_int), ('x', C.c_void_p), ('x_stride', C.c_int64 * 4),
+                ('y', C.c_void_p), ('y_stride', C.c_int64 * 4), ('lin', C.c_void_p),
+                ('grad_x', C.c_void_p), ('gx_stride', C.c_int64 * 4), ('grad_y', C.c_void_p), ('gy_stride', C.c_int64 * 4)]
+
+
+class LpipsParams(C.Structure):
+    _fields_ = [('n', C.c_int), ('num_layers', C.c_int), ('layers', LpipsLayer * LPIPS_MAX_LAYERS), ('value', C.c_void_p),
+                ('scratch', C.c_void_p), ('scratch_bytes', C.c_int64), ('grad_value', C.c_void_p)]
+
+
 _lib = None
 
 
@@ -212,10 +226,14 @@ def get_lib():
     lib.ide3d_noise_normalize.argtypes = [C.POINTER(NoiseTable), vp]
     lib.ide3d_seg_xent_fwd.argtypes = [C.POINTER(SegXentParams), vp]
     lib.ide3d_seg_xent_bwd.argtypes = [C.POINTER(SegXentParams), vp]
+    lib.ide3d_lpips_scratch_bytes.argtypes = [C.POINTER(LpipsParams)]
+    lib.ide3d_lpips_scratch_bytes.restype = C.c_int64
+    lib.ide3d_lpips_fwd.argtypes = [C.POINTER(LpipsParams), vp]
+    lib.ide3d_lpips_bwd.argtypes = [C.POINTER(LpipsParams), vp]
     for name in ('bias_act', 'upfirdn2d', 'filtered_lrelu', 'filtered_lrelu_act', 'raymarch_fwd', 'raymarch_bwd', 'raymarch_bwd_cam', 'sample_voxel',
                  'sigma_grid', 'planes_to_nhwc', 'initial_rays', 'transform_points', 'sample_triplane', 'integrate',
                  'sample_pdf', 'style_plan', 'mc_classify', 'mc_emit', 'mesh_normals', 'raster', 'video_frames', 'image_strips',
-                 'noise_reg', 'noise_normalize', 'seg_xent_fwd', 'seg_xent_bwd', 'abi_version'):
+                 'noise_reg', 'noise_normalize', 'seg_xent_fwd', 'seg_xent_bwd', 'lpips_fwd', 'lpips_bwd', 'abi_version'):
         getattr(lib, 'ide3d_' + name).restype = C.c_int
     if lib.ide3d_abi_version() != 1:
         raise RuntimeError('ide3d_b200: ABI version mismatch between _lib.py and libide3d_b200.so')
@@ -231,7 +249,8 @@ def exported_symbols():
             'ide3d_sigma_grid', 'ide3d_planes_to_nhwc', 'ide3d_initial_rays', 'ide3d_transform_points',
             'ide3d_sample_triplane', 'ide3d_integrate', 'ide3d_sample_pdf', 'ide3d_mask2color', 'ide3d_style_plan', 'ide3d_mc_classify', 'ide3d_mc_emit',
             'ide3d_mesh_normals', 'ide3d_raster_scratch_bytes', 'ide3d_raster', 'ide3d_video_frames', 'ide3d_image_strips',
-            'ide3d_noise_reg', 'ide3d_noise_normalize', 'ide3d_seg_xent_fwd', 'ide3d_seg_xent_bwd']
+            'ide3d_noise_reg', 'ide3d_noise_normalize', 'ide3d_seg_xent_fwd', 'ide3d_seg_xent_bwd',
+            'ide3d_lpips_scratch_bytes', 'ide3d_lpips_fwd', 'ide3d_lpips_bwd']
 
 
 def check(rc, allow_unsupported=False):

@@ -142,6 +142,19 @@ class TriPlaneRenderer(torch.nn.Module):
                                return_weights=return_weights, views=views)
 
 
+def invalidate_caches(module):
+    """Drop every inference constant cached under `module`: SynthesisLayer's noise products and transposed weights, the synthesis
+    networks' style plans and the renderers' packed decoders; each is rebuilt on its next use.  Those caches key on
+    (data_ptr, _version) of the parameters, and an in-place update that does not bump _version (torch.optim.Adam(fused=True) does
+    not) leaves them stale: call this after changing weights that way."""
+    for m in module.modules():
+        m.__dict__.pop('_const_cache', None)
+        if isinstance(m, SynthesisNetwork):
+            _STYLE_PLANS.pop(m, None)
+        if isinstance(m, TriPlaneRenderer):
+            m._packed = m._packed_key = None
+
+
 # ================================================================================================ synthesis
 def upsample_seg(seg_raw, size):
     """Render-resolution semantic logits [N, 19, R, R] -> image resolution: bilinear, align_corners=False.  The rule of

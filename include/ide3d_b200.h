@@ -29,6 +29,7 @@
  *   ide3d_noise_reg           inversion/training/projectors/w_projector_ide3d.py:113-122  noise regulariser (+ its gradient)
  *   ide3d_noise_normalize     inversion/training/projectors/w_projector_ide3d.py:138-142  noise renormalisation
  *   ide3d_seg_xent_fwd/_bwd   semantic-mask loss of the projector (extension): cross-entropy of the upsampled logits
+ *   ide3d_lpips_fwd/_bwd      inversion/criteria/lpips/lpips.py:29-35 + utils.py:6-8  LPIPS head over all tapped layers (pivotal tuning)
  *
  * Conventions
  *   - plain C: raw device pointers, sizes, strides (in ELEMENTS), a cudaStream_t passed as void*.
@@ -495,6 +496,48 @@ typedef struct ide3d_seg_xent_params {
 } ide3d_seg_xent_params;
 int ide3d_seg_xent_fwd(const ide3d_seg_xent_params* p, ide3d_stream_t stream);
 int ide3d_seg_xent_bwd(const ide3d_seg_xent_params* p, ide3d_stream_t stream);
+
+/* LPIPS v0.1 head of pivotal tuning (inversion/criteria/lpips/{lpips,utils}.py, the pip `lpips` package) over every tapped layer of
+ * one call.  Per layer l, sample n and pixel p, with the norm over the channels:
+ *   u = x / (||x||_2 + 1e-10),  v = y / (||y||_2 + 1e-10),  value[n] = sum_l mean_p sum_c lin_l[c] * (u_c - v_c)^2
+ * x, y fp32 [n, c, h, w] with any element strides (NCHW and channels_last both coalesce on their fastest axis); y may have
+ * y_stride[0] = 0 (one target for every sample).
+ *   ide3d_lpips_fwd: value[n] (float) and, in scratch, the per-block partial sums and the per-(sample, layer) values (double, at
+ *                    scratch + ide3d_lpips_scratch_bytes - 8 * n * num_layers, sample-major).  Two launches whatever num_layers:
+ *                    one CTA per (layer, sample, 256 pixels) sums its pixels in double in a fixed order, one more launch folds the
+ *                    partials per sample and layer in block order, then the layers in order.  No float atomics: deterministic.
+ *   ide3d_lpips_bwd: one launch.  With g_c = grad_value[n] * (2 / (h w)) * lin[c] * (u_c - v_c) and s = 1 / (||x|| + 1e-10):
+ *                      grad_x_k = s g_k - (s^2 / ||x||) x_k sum_c g_c x_c        (grad_y likewise with -g_c and y)
+ *                    grad_x / grad_y use their own strides and may be NULL (not wanted); grad_y is per sample (gy_stride[0] != 0
+ *                    when n > 1): a broadcast target's gradient is the caller's sum over n.
+ *                    At a pixel whose vector is exactly zero the gradient written is 0.  torch's autograd gives NaN there (the
+ *                    derivative of sqrt at 0); 0 keeps a ReLU trunk's gradient finite, as torch's threshold_backward makes it.
+ * IDE3D_UNSUPPORTED for num_layers > IDE3D_LPIPS_MAX_LAYERS; IDE3D_INVALID for null pointers, empty sizes or offsets beyond 31 bits. */
+#define IDE3D_LPIPS_MAX_LAYERS 8
+typedef struct ide3d_lpips_layer {
+    int c, h, w;
+    const float* x;
+    int64_t x_stride[4];        /* n, c, h, w */
+    const float* y;
+    int64_t y_stride[4];
+    const float* lin;           /* [c] */
+    float* grad_x;              /* bwd, optional */
+    int64_t gx_stride[4];
+    float* grad_y;              /* bwd, optional */
+    int64_t gy_stride[4];
+} ide3d_lpips_layer;
+typedef struct ide3d_lpips_params {
+    int n, num_layers;
+    ide3d_lpips_layer layers[IDE3D_LPIPS_MAX_LAYERS];
+    float* value;               /* fwd: [n] */
+    void* scratch;              /* fwd: ide3d_lpips_scratch_bytes(p) bytes, 8-byte aligned */
+    int64_t scratch_bytes;
+    const float* grad_value;    /* bwd: [n] */
+} ide3d_lpips_params;
+/* bytes of scratch ide3d_lpips_fwd needs for this table (negative status for a table it would refuse) */
+int64_t ide3d_lpips_scratch_bytes(const ide3d_lpips_params* p);
+int ide3d_lpips_fwd(const ide3d_lpips_params* p, ide3d_stream_t stream);
+int ide3d_lpips_bwd(const ide3d_lpips_params* p, ide3d_stream_t stream);
 
 #ifdef __cplusplus
 }
