@@ -195,6 +195,8 @@ def get_lib():
     vp, i32, i64, f32 = C.c_void_p, C.c_int, C.c_int64, C.c_float
     lib.ide3d_bias_act.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, f32, f32, f32, i64, i64, i64, vp]
     lib.ide3d_modconv_epilogue.argtypes = [vp, vp, vp, vp, vp, vp, vp, i32, i32, f32, f32, f32, i64, i64, i64, i64, i32, vp]
+    lib.ide3d_modconv_epilogue_rgb.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i64, i32, i32, f32, f32, f32, i64, i64, i64,
+                                               i64, vp]
     lib.ide3d_upfirdn2d.argtypes = [C.POINTER(UpfirParams), vp]
     lib.ide3d_upfirdn2d_add.argtypes = [C.POINTER(UpfirParams), vp, i64, i64, i64, vp, vp]
     lib.ide3d_upfirdn2d_epilogue.argtypes = [C.POINTER(UpfirParams), C.POINTER(FirEpilogue), vp]
@@ -243,7 +245,7 @@ def get_lib():
 
 def exported_symbols():
     """Names declared in include/ide3d_b200.h (used by the CPU test that checks the .so exports them)."""
-    return ['ide3d_abi_version', 'ide3d_last_error', 'ide3d_launch_count', 'ide3d_bias_act', 'ide3d_modconv_epilogue',
+    return ['ide3d_abi_version', 'ide3d_last_error', 'ide3d_launch_count', 'ide3d_bias_act', 'ide3d_modconv_epilogue', 'ide3d_modconv_epilogue_rgb',
             'ide3d_upfirdn2d', 'ide3d_upfirdn2d_add', 'ide3d_upfirdn2d_epilogue',
             'ide3d_filtered_lrelu', 'ide3d_filtered_lrelu_act', 'ide3d_raymarch_fwd', 'ide3d_raymarch_bwd', 'ide3d_raymarch_bwd_cam', 'ide3d_sample_voxel',
             'ide3d_sigma_grid', 'ide3d_planes_to_nhwc', 'ide3d_initial_rays', 'ide3d_transform_points',

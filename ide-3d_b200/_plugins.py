@@ -103,6 +103,61 @@ def modconv_epilogue(x, scale, noise, b, act, alpha, gain, clamp, next_scale=Non
     return y2 if y is None else (y, y2)
 
 
+def modconv_epilogue_rgb(x, scale, noise, b, act, alpha, gain, clamp, emit_y=True, y_scale=None, next_scale=None, rgb=None):
+    """`modconv_epilogue` for channels_last float32 x with the consumers of its output folded in (extension, forward only):
+    y = t (* y_scale[:, :, None, None]) if emit_y; y2 = t * next_scale[:, :, None, None] if next_scale is given; with
+    rgb = (weight [O,C,1,1], styles [N,C], bias [O] | None), O <= 4, the ToRGB output conv1x1(t * styles, weight) + bias as a dense
+    NCHW [N,O,H,W] tensor.  Returns the list of the requested outputs in the order (y, y2, rgb), or None when the kernel does
+    not take the shape (caller composes the reference ops instead)."""
+    L.require_cuda(x)
+    _req(x.ndim == 4, 'x must be rank 4')
+    n, c, h, w = x.shape
+    cl = (not x.is_contiguous()) and x.is_contiguous(memory_format=torch.channels_last)
+    if not cl or x.dtype != torch.float32 or c % 4 != 0 or c > 512 or x.numel() == 0:
+        return None
+
+    def per_sample(t, name):
+        if not _has(t):
+            return None
+        _req(t.numel() == n * c, f'{name} must have N*C elements')
+        return t.to(dtype=x.dtype).reshape(n, c).contiguous()
+
+    scale, y_scale, next_scale = per_sample(scale, 'scale'), per_sample(y_scale, 'y_scale'), per_sample(next_scale, 'next_scale')
+    noise_batch = 1
+    if _has(noise):
+        _req(noise.numel() in (h * w, n * h * w), 'noise must be [H,W] or [N,1,H,W]')
+        noise_batch = noise.numel() // (h * w)
+        noise = noise.to(dtype=x.dtype).contiguous()
+    if _has(b):
+        _req(b.ndim == 1 and b.shape[0] == c, 'b has wrong number of elements')
+        b = b.to(dtype=x.dtype).contiguous()
+    _req(y_scale is None or emit_y, 'y_scale needs emit_y')
+    wrgb = srgb = brgb = out_rgb = None
+    o = 0
+    if rgb is not None:
+        wrgb, srgb, brgb = rgb
+        o = wrgb.shape[0]
+        if o > 4:
+            return None
+        _req(wrgb.numel() == o * c, 'rgb weight must be [O, C, 1, 1]')
+        wrgb = wrgb.to(dtype=x.dtype).reshape(o, c).contiguous()
+        srgb = per_sample(srgb, 'rgb styles')
+        if brgb is not None:
+            _req(brgb.numel() == o, 'rgb bias must have O elements')
+            brgb = brgb.to(dtype=x.dtype).contiguous()
+        out_rgb = torch.empty([n, o, h, w], dtype=x.dtype, device=x.device)
+    y = torch.empty_like(x) if emit_y else None
+    y2 = torch.empty_like(x) if next_scale is not None else None
+    _req(y is not None or y2 is not None or out_rgb is not None, 'no output requested')
+    opt = lambda t: L.ptr(t) if t is not None else None
+    rc = L.get_lib().ide3d_modconv_epilogue_rgb(L.ptr(x), opt(scale), opt(noise), opt(b), opt(y_scale), opt(y), opt(next_scale), opt(y2),
+                                                opt(wrgb), opt(srgb), opt(brgb), opt(out_rgb), o, L.dtype_code(x), int(act), float(alpha),
+                                                float(gain), float(clamp), n, c, h * w, noise_batch, L.stream_ptr(x.device))
+    if L.check(rc, allow_unsupported=True) == L.UNSUPPORTED:
+        return None
+    return [t for t in (y, y2, out_rgb) if t is not None]
+
+
 # ------------------------------------------------------------------------------------------- upfirdn2d
 def upfirdn2d(x, f, upx, upy, downx, downy, padx0, padx1, pady0, pady1, flip, gain, add=None, bias=None, epilogue=None):
     """Extensions (return None if the kernel cannot fuse them, so the caller composes the reference ops):
@@ -260,7 +315,8 @@ class _Plugin:
 
 
 PLUGINS = {
-    'bias_act_plugin': _Plugin('bias_act_plugin', bias_act=bias_act, modconv_epilogue=modconv_epilogue),
+    'bias_act_plugin': _Plugin('bias_act_plugin', bias_act=bias_act, modconv_epilogue=modconv_epilogue,
+                                 modconv_epilogue_rgb=modconv_epilogue_rgb),
     'upfirdn2d_plugin': _Plugin('upfirdn2d_plugin', upfirdn2d=upfirdn2d),
     'filtered_lrelu_plugin': _Plugin('filtered_lrelu_plugin', filtered_lrelu=filtered_lrelu,
                                      filtered_lrelu_act_=filtered_lrelu_act_),

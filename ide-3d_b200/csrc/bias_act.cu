@@ -496,3 +496,193 @@ extern "C" int ide3d_modconv_epilogue(const void* x, const void* scale, const vo
     }
     IDE3D_FAIL(IDE3D_INVALID, "modconv_epilogue: unsupported dtype %d", dtype);
 }
+
+// ------------------------------------------------------------------------------------------------------------------
+// The channels_last fp32 epilogue with the next consumers folded in: besides t = bias_act(x * scale + noise, b) it writes any of
+//   y   = t (* yscale[n,c])          the plain output, or already the next block's `x * styles` (inversion/networks.py:100)
+//   y2  = t * scale2[n,c]            the next layer's `x * styles`, as ide3d_modconv_epilogue
+//   rgb = sum_c wrgb[o,c] srgb[n,c] t_c + brgb[o]   (o < 4, dense NCHW)   the ToRGB layer of the block (:700-707): a modulated 1x1
+//         convolution without demodulation, i.e. a 3 x C dot product per pixel -- 3 FMAs per 4 bytes read, far below the FMA:byte
+//         ratio of the machine, so the pass stays an HBM stream and the x * s_rgb tensor and the 1x1 convolution disappear.
+// Thread mapping: the 256 threads of a block cover ppb = 256 / (C/4) whole pixels per pass, each thread one 16-byte vector of one
+// pixel, the same vector of every pixel it visits -- so its slice of every per-channel operand (scale, b, yscale, scale2 and the
+// modulated ToRGB weights wrgb * srgb of the sample) is formed once per sample and kept in registers.  Reduction of a pixel's
+// partial dot products: an xor-shuffle butterfly over its lanes when C/4 is a power of two <= 32 (the lanes of a pixel are then an
+// aligned group of one warp), else the partials go through shared memory and one thread per (pixel, o) adds them in lane order.
+// Either way the order is fixed and there are no atomics: reruns are bit-identical.
+namespace ide3d {
+
+constexpr int kRgbMax = 4;
+
+struct EpiRgbArgs {
+    const float *x, *scale, *noise, *b;
+    const float* yscale;
+    float* y;
+    const float* scale2;
+    float* y2;
+    const float *wrgb, *srgb, *brgb;
+    float* rgb;
+    float alpha, gain, clamp;
+    int n, c, hw, o;
+    int noise_batch;
+};
+
+__device__ __forceinline__ void load4(const float* p, long long v, float (&o)[4]) {
+    const float4 t = __ldg(reinterpret_cast<const float4*>(p) + v);
+    o[0] = t.x; o[1] = t.y; o[2] = t.z; o[3] = t.w;
+}
+
+template <int A, bool kShfl>
+__global__ void __launch_bounds__(256) modconv_epilogue_rgb_cl_kernel(const EpiRgbArgs p, int ppb, unsigned chunks_per_sample,
+                                                                     long long items) {
+    constexpr int UNROLL = 4;
+    __shared__ float part[kShfl ? 1 : 256 * kRgbMax];
+    const unsigned cv = (unsigned)p.c >> 2;                       // vectors per pixel
+    const unsigned lp = threadIdx.x / cv, c0 = threadIdx.x - lp * cv;
+    const bool lane_on = (int)lp < ppb;
+    const bool want_rgb = p.rgb != nullptr;
+    const unsigned svec = (unsigned)p.hw * cv;
+    int cur = -1;
+    float d[4], bb[4], ys[4], s2[4], wr[kRgbMax][4];
+    for (long long item = blockIdx.x; item < items; item += gridDim.x) {
+        const int smp = (int)(item / chunks_per_sample);
+        const unsigned chunk = (unsigned)(item - (long long)smp * chunks_per_sample);
+        if (smp != cur && lane_on) {                               // per-sample operands of this thread's 4 channels
+            cur = smp;
+            const long long sv = (long long)smp * cv + c0;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) d[j] = bb[j] = ys[j] = s2[j] = 1.f;
+            if (p.scale) load4(p.scale, sv, d);
+            if (p.b) load4(p.b, c0, bb);
+            if (p.yscale) load4(p.yscale, sv, ys);
+            if (p.y2) load4(p.scale2, sv, s2);
+#pragma unroll
+            for (int o = 0; o < kRgbMax; ++o)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const int ch = (int)(4 * c0) + j;
+                    wr[o][j] = (want_rgb && o < p.o) ? __ldg(p.wrgb + (long long)o * p.c + ch) * __ldg(p.srgb + (long long)smp * p.c + ch) : 0.f;
+                }
+        }
+        const long long vbase = (long long)smp * svec;
+        const unsigned pix0 = chunk * (unsigned)(ppb * UNROLL);
+        float vx[UNROLL][4];
+#pragma unroll
+        for (int u = 0; u < UNROLL; ++u) {
+            const unsigned pix = pix0 + u * ppb + lp;
+            if (lane_on && pix < (unsigned)p.hw) load_vec(p.x, vbase + pix * cv + c0, vx[u]);
+        }
+#pragma unroll
+        for (int u = 0; u < UNROLL; ++u) {
+            const unsigned pix = pix0 + u * ppb + lp;
+            const bool ok = lane_on && pix < (unsigned)p.hw;
+            float acc[kRgbMax] = {0.f, 0.f, 0.f, 0.f};
+            if (ok) {
+                const float nz = p.noise ? __ldg(p.noise + (p.noise_batch == 1 ? (long long)pix : (long long)smp * p.hw + pix)) : 0.f;
+                float t[4], out[4];
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    float v = p.scale ? vx[u][j] * d[j] : vx[u][j];
+                    if (p.noise) v = p.scale ? vx[u][j] * d[j] + nz : vx[u][j] + nz;
+                    t[j] = eval<float, A>(v, p.b ? bb[j] : 0.f, 0.f, 0.f, 1.f, 0, p.alpha, p.gain, p.clamp);
+                }
+                const long long v = vbase + pix * cv + c0;
+                if (p.y) {
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) out[j] = p.yscale ? t[j] * ys[j] : t[j];
+                    store_vec(p.y, v, out);
+                }
+                if (p.y2) {
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) out[j] = t[j] * s2[j];
+                    store_vec(p.y2, v, out);
+                }
+                if (want_rgb) {
+#pragma unroll
+                    for (int o = 0; o < kRgbMax; ++o) acc[o] = ((wr[o][0] * t[0] + wr[o][1] * t[1]) + wr[o][2] * t[2]) + wr[o][3] * t[3];
+                }
+            }
+            if (!want_rgb) continue;                               // block-uniform
+            if constexpr (kShfl) {
+                for (unsigned m = 1; m < cv; m <<= 1)
+#pragma unroll
+                    for (int o = 0; o < kRgbMax; ++o) acc[o] += __shfl_xor_sync(0xffffffffu, acc[o], m);
+                if (ok)                                            // every lane holds the sums; lane c0 writes outputs c0, c0 + C/4, ...
+                    for (int o = (int)c0; o < p.o; o += (int)cv) {
+                        const float r = o == 0 ? acc[0] : o == 1 ? acc[1] : o == 2 ? acc[2] : acc[3];
+                        p.rgb[((long long)smp * p.o + o) * p.hw + pix] = p.brgb ? r + __ldg(p.brgb + o) : r;
+                    }
+            } else {
+#pragma unroll
+                for (int o = 0; o < kRgbMax; ++o) part[threadIdx.x * kRgbMax + o] = acc[o];
+                __syncthreads();
+                if ((int)threadIdx.x < ppb * p.o) {
+                    const int q = (int)threadIdx.x / p.o, o = (int)threadIdx.x - q * p.o;
+                    const unsigned qpix = pix0 + u * ppb + q;
+                    if (qpix < (unsigned)p.hw) {
+                        float r = 0.f;
+                        for (unsigned k = 0; k < cv; ++k) r += part[(q * cv + k) * kRgbMax + o];
+                        p.rgb[((long long)smp * p.o + o) * p.hw + qpix] = p.brgb ? r + __ldg(p.brgb + o) : r;
+                    }
+                }
+                __syncthreads();
+            }
+        }
+    }
+}
+
+template <int A>
+static int launch_epilogue_rgb(const EpiRgbArgs& p, cudaStream_t st) {
+    constexpr int UNROLL = 4;
+    const int cv = p.c / 4;
+    const bool shfl = cv <= 32 && (cv & (cv - 1)) == 0;
+    const int ppb = 256 / cv;
+    const long long cps = ceil_div<long long>(p.hw, (long long)ppb * UNROLL);
+    const long long items = (long long)p.n * cps;
+    const long long cap = (long long)sm_count() * 8;
+    const long long blocks = items < cap ? items : cap;
+    if (shfl) modconv_epilogue_rgb_cl_kernel<A, true><<<(unsigned)blocks, 256, 0, st>>>(p, ppb, (unsigned)cps, items);
+    else modconv_epilogue_rgb_cl_kernel<A, false><<<(unsigned)blocks, 256, 0, st>>>(p, ppb, (unsigned)cps, items);
+    IDE3D_CHECK_LAUNCH("modconv_epilogue_rgb_cl_kernel");
+    return IDE3D_OK;
+}
+
+}  // namespace ide3d
+
+extern "C" int ide3d_modconv_epilogue_rgb(const void* x, const void* scale, const void* noise, const void* b, const void* yscale,
+                                          void* y, const void* scale2, void* y2, const void* wrgb, const void* srgb, const void* brgb,
+                                          void* rgb, int64_t rgb_channels, int dtype, int act, float alpha, float gain, float clamp,
+                                          int64_t n, int64_t c, int64_t hw, int64_t noise_batch, ide3d_stream_t stream) {
+    IDE3D_REQUIRE(n >= 0 && c >= 0 && hw >= 0, "modconv_epilogue_rgb: negative size");
+    if (n * c * hw == 0) return IDE3D_OK;
+    IDE3D_REQUIRE(x && (y || y2 || rgb), "modconv_epilogue_rgb: null x / no output");
+    IDE3D_REQUIRE((y2 == nullptr) == (scale2 == nullptr), "modconv_epilogue_rgb: scale2 and y2 go together");
+    IDE3D_REQUIRE(yscale == nullptr || y != nullptr, "modconv_epilogue_rgb: yscale without y");
+    IDE3D_REQUIRE(rgb == nullptr || (wrgb && srgb && rgb_channels >= 1 && rgb_channels <= kRgbMax),
+                  "modconv_epilogue_rgb: rgb needs wrgb, srgb and 1..4 output channels");
+    IDE3D_REQUIRE(noise == nullptr || noise_batch == 1 || noise_batch == n, "modconv_epilogue_rgb: noise batch must be 1 or n");
+    IDE3D_REQUIRE(act >= 1 && act <= 9, "modconv_epilogue_rgb: unknown activation index %d", act);
+    const uintptr_t all = (uintptr_t)x | (uintptr_t)y | (uintptr_t)scale | (uintptr_t)b | (uintptr_t)yscale | (uintptr_t)scale2 | (uintptr_t)y2;
+    IDE3D_REQUIRE((all & 15) == 0, "modconv_epilogue_rgb: x, y, y2 and the per-channel operands must be 16-byte aligned");
+    IDE3D_REQUIRE((((uintptr_t)noise | (uintptr_t)wrgb | (uintptr_t)srgb | (uintptr_t)brgb | (uintptr_t)rgb) & 3) == 0,
+                  "modconv_epilogue_rgb: noise / ToRGB operands must be 4-byte aligned");
+    if (dtype != IDE3D_F32) IDE3D_FAIL(IDE3D_UNSUPPORTED, "modconv_epilogue_rgb: float32 only");
+    if (c % 4 != 0 || c > 512) IDE3D_FAIL(IDE3D_UNSUPPORTED, "modconv_epilogue_rgb: needs C %% 4 == 0 and C <= 512 (got %lld)", (long long)c);
+    if (hw * (c / 4) >= (1ll << 31) || n >= (1ll << 31)) IDE3D_FAIL(IDE3D_UNSUPPORTED, "modconv_epilogue_rgb: more than 2^31 vectors per sample");
+    ide3d::EpiRgbArgs p{(const float*)x, (const float*)scale, (const float*)noise, (const float*)b, (const float*)yscale, (float*)y,
+                        (const float*)scale2, (float*)y2, (const float*)wrgb, (const float*)srgb, (const float*)brgb, (float*)rgb,
+                        alpha, gain, clamp, (int)n, (int)c, (int)hw, rgb ? (int)rgb_channels : 0, (int)noise_batch};
+    cudaStream_t st = (cudaStream_t)stream;
+    switch (act) {
+        case 1: return ide3d::launch_epilogue_rgb<1>(p, st);
+        case 2: return ide3d::launch_epilogue_rgb<2>(p, st);
+        case 3: return ide3d::launch_epilogue_rgb<3>(p, st);
+        case 4: return ide3d::launch_epilogue_rgb<4>(p, st);
+        case 5: return ide3d::launch_epilogue_rgb<5>(p, st);
+        case 6: return ide3d::launch_epilogue_rgb<6>(p, st);
+        case 7: return ide3d::launch_epilogue_rgb<7>(p, st);
+        case 8: return ide3d::launch_epilogue_rgb<8>(p, st);
+        case 9: return ide3d::launch_epilogue_rgb<9>(p, st);
+    }
+    IDE3D_FAIL(IDE3D_INVALID, "modconv_epilogue_rgb: unknown activation index %d", act);
+}

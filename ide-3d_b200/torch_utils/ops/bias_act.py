@@ -133,17 +133,23 @@ def bias_act(x, b=None, dim=1, act='linear', alpha=None, gain=None, clamp=None, 
 
 
 def scaled_bias_act(x, scale=None, noise=None, b=None, act='linear', alpha=None, gain=None, clamp=None, next_scale=None,
-                    only_next=False):
+                    only_next=False, emit_y=True, y_scale=None, rgb=None):
     """Extension: ``bias_act(fma(x, scale[:, :, None, None], noise), b, act=...)`` -- the tail of an activation-scaled
     modulated convolution (inversion/networks.py:104-105 then :512) -- as ONE sm_90a pass when nothing needs a gradient;
     otherwise exactly that composition of the two reference ops (so autograd behaves as in the reference).
     x [N,C,H,W]; scale [N,C] (demodulation coefficients) | None; noise broadcastable [.,1,H,W] | None; b [C] | None.
     next_scale [N,C]: additionally return ``y * next_scale[:, :, None, None]`` (the style modulation that opens the next
-    modulated convolution, :100) -> (y, y_next); with only_next just y_next."""
+    modulated convolution, :100) -> (y, y_next); with only_next just y_next.
+    Further consumers folded into the same pass: emit_y=False drops y (as only_next), y_scale [N,C] returns ``y * y_scale``
+    in place of y (the next block's first modulation), rgb=(weight [O,C,1,1], styles [N,C], bias [O] | None) adds the ToRGB
+    output ``conv1x1(y * styles, weight) + bias`` as a dense NCHW tensor (ToRGBLayer, :700-707).  With any of these the
+    result is the list of the requested outputs in the order (y, y2, rgb)."""
     from . import fma
     if x.device.type != 'cuda':
         raise RuntimeError('ide3d_b200.scaled_bias_act: x must be a CUDA tensor (no CPU path in this package)')
     _init()
+    if rgb is not None or y_scale is not None or not emit_y:
+        return _scaled_bias_act_fold(x, scale, noise, b, act, alpha, gain, clamp, next_scale, emit_y and not only_next, y_scale, rgb)
     spec = activation_funcs[act]
     needs_grad = torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (x, scale, noise, b, next_scale))
     if not needs_grad and x.ndim == 4:
@@ -163,3 +169,33 @@ def scaled_bias_act(x, scale=None, noise=None, b=None, act='linear', alpha=None,
         return y
     y2 = y * next_scale.to(y.dtype).reshape(y.shape[0], -1, 1, 1)
     return y2 if only_next else (y, y2)
+
+
+def _scaled_bias_act_fold(x, scale, noise, b, act, alpha, gain, clamp, next_scale, emit_y, y_scale, rgb):
+    """`scaled_bias_act` with its consumers folded in: one `ide3d_modconv_epilogue_rgb` pass for channels_last float32 inference;
+    for anything else (gradients, other layouts / dtypes / widths) today's composition -- the epilogue, the products with the
+    styles and, for rgb, the cuDNN 1x1 convolution followed by the bias."""
+    from . import conv2d_resample
+    spec = activation_funcs[act]
+    alpha = float(alpha if alpha is not None else spec.def_alpha)
+    gain = float(gain if gain is not None else spec.def_gain)
+    clamp_f = float(clamp if clamp is not None else -1)
+    needs_grad = torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (x, scale, noise, b, next_scale, y_scale, *(rgb or ())))
+    if not needs_grad and x.ndim == 4:
+        out = _plugin.modconv_epilogue_rgb(x, scale, noise, b, spec.cuda_idx, alpha, gain, clamp_f, emit_y=emit_y, y_scale=y_scale,
+                                           next_scale=next_scale, rgb=rgb)
+        if out is not None:
+            return out
+    y = scaled_bias_act(x, scale, noise, b, act=act, alpha=alpha, gain=gain, clamp=clamp)
+    mod = lambda s: y * s.to(y.dtype).reshape(y.shape[0], -1, 1, 1)
+    out = []
+    if emit_y:
+        out.append(y if y_scale is None else mod(y_scale))
+    if next_scale is not None:
+        out.append(mod(next_scale))
+    if rgb is not None:
+        weight, styles, bias = rgb
+        r = conv2d_resample.conv2d_resample(x=mod(styles), w=weight.to(y.dtype))
+        r = bias_act(r, None if bias is None else bias.to(r.dtype))
+        out.append(r.contiguous())
+    return out

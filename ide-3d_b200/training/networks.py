@@ -28,6 +28,10 @@ FUSED_MODCONV_MIN_RES = 1 << 30      # block resolutions >= this use the grouped
 CHANNELS_LAST = os.environ.get('IDE3D_CHANNELS_LAST', '1') != '0'
 STYLE_PLAN = os.environ.get('IDE3D_STYLE_PLAN', '1') != '0'      # styles + demodulation coefficients of a whole synthesis call in two launches (StylePlan)
 CHAIN_MODULATION = True              # epilogues also write the next layer's `x * styles` (SynthesisBlock._features)
+# fp32 NHWC inference without conv_clamp: the last epilogue of a block also computes its ToRGB output (<= 4 channels) and, inside a
+# synthesis call, writes the next block's `x * styles` instead of x (nothing at all for the last block).  IDE3D_FUSED_TORGB=0 restores
+# the separate passes (x * s_rgb, cuDNN 1x1 convolution, bias, x * s0 of the next block) for A/B runs.
+FUSED_TORGB = os.environ.get('IDE3D_FUSED_TORGB', '1') != '0'
 # 1x1 convolutions of NHWC activations as one [N*H*W, I] x [I, O] matrix product (cuBLASLt, tf32 exactly when the cuDNN convolution
 # it replaces would use tf32) instead of cuDNN's conv3d_fprop kernels, which stream these shapes at ~40 % of the HBM peak.
 # Off by default; kept as a switch for A/B runs.
@@ -218,9 +222,11 @@ class SynthesisLayer(torch.nn.Module):
         self.bias = torch.nn.Parameter(torch.zeros([out_channels]))
 
     def forward(self, x, w, noise_mode='random', fused_modconv=True, gain=1, styles=None, premodulated=False, next_styles=None,
-                only_next=False, dcoefs=None):
+                only_next=False, dcoefs=None, y_styles=None, emit_y=True, rgb=None):
         """styles / premodulated / next_styles / only_next: block-internal chaining of activation-scaled layers -- the
-        epilogue of this layer can already write `y * next_styles` for the layer that follows (see SynthesisBlock._features)."""
+        epilogue of this layer can already write `y * next_styles` for the layer that follows (see SynthesisBlock._features).
+        y_styles / emit_y / rgb (3x3 layers without upsampling): the epilogue returns `y * y_styles` in place of y, or no y,
+        and the ToRGB output of rgb = (weight, styles, bias) -- `bias_act.scaled_bias_act`."""
         assert noise_mode in ['random', 'const', 'none']
         if styles is None:
             styles = self.affine(w)
@@ -239,6 +245,12 @@ class SynthesisLayer(torch.nn.Module):
         epilogue = dict(b=self.bias, act=self.activation, gain=act_gain, clamp=act_clamp)
         if next_styles is not None:
             epilogue.update(next_scale=next_styles, only_next=only_next)
+        if y_styles is not None:
+            epilogue['y_scale'] = y_styles
+        if not emit_y:
+            epilogue['emit_y'] = False
+        if rgb is not None:
+            epilogue['rgb'] = rgb
         w_t = None
         if inference and self.up > 1 and not fused_modconv and x.dtype == self.weight.dtype:
             fmt = torch.channels_last if CHANNELS_LAST else torch.contiguous_format
@@ -313,8 +325,20 @@ class SynthesisBlock(torch.nn.Module):
                                 channels_last=self.channels_last or CHANNELS_LAST)
         self.num_torgb += 1
 
+    def can_fold(self):
+        """Can this block's epilogues take over its neighbours' passes (FUSED_TORGB)?  Only for the NHWC layout and without
+        conv_clamp; the caller still needs the block on the chained path (fp32 inference, activation scaling)."""
+        return FUSED_TORGB and CHAIN_MODULATION and CHANNELS_LAST and self.conv1.conv_clamp is None and self.torgb.conv_clamp is None
+
     def _features(self, x, ws, force_fp32, fused_modconv, layer_kwargs):
+        """-> (x, w_rgb, fused_modconv, rgb_in, y_rgb).  Keys of layer_kwargs a synthesis network uses to chain its blocks (each
+        needs the chained path below): premodulated_x -- x already carries conv0's styles (the previous block's epilogue wrote
+        them); x_next_styles [N, C] -- return `x * x_next_styles` (the next block's conv0 styles) instead of x; drop_x -- return
+        no x (nothing consumes it).  y_rgb is the ToRGB output (bias included) when conv1's epilogue computed it."""
         layer_kwargs = dict(layer_kwargs)
+        premod_in = layer_kwargs.pop('premodulated_x', False)
+        x_next_styles = layer_kwargs.pop('x_next_styles', None)
+        drop_x = layer_kwargs.pop('drop_x', False)
         misc.assert_shape(ws, [None, self.num_conv + self.num_torgb, self.w_dim])
         w_iter = iter(ws.unbind(dim=1))
         dtype = torch.float16 if self.use_fp16 and not force_fp32 else torch.float32
@@ -330,7 +354,9 @@ class SynthesisBlock(torch.nn.Module):
         # separate modulation passes of conv1 and ToRGB disappear (conv0 -> x*s1 only; conv1 -> x and x*s_rgb).
         chain = CHAIN_MODULATION and (not fused_modconv) and dtype == torch.float32 and not (torch.is_grad_enabled() and (
             ws.requires_grad or any(p.requires_grad for p in self.parameters())))
-        rgb_in = None
+        if not chain and (premod_in or x_next_styles is not None or drop_x):
+            raise RuntimeError('SynthesisBlock: cross-block chaining needs the chained fp32 inference path')
+        rgb_in = y_rgb = None
         if self.in_channels == 0:
             x = self.const.to(dtype=dtype).unsqueeze(0).repeat([ws.shape[0], 1, 1, 1]).contiguous(memory_format=memory_format)
             w1 = next(w_iter)
@@ -349,15 +375,30 @@ class SynthesisBlock(torch.nn.Module):
                 s1, s_rgb, s0, d0, d1 = self.conv1.affine(w1), self.torgb.styles(w_rgb), None, None, None
             pre = False
             if self.in_channels != 0:
-                x = self.conv0(x, w0, fused_modconv=False, styles=s0, dcoefs=d0, next_styles=s1, only_next=True, **layer_kwargs)
+                x = self.conv0(x, w0, fused_modconv=False, styles=s0, dcoefs=d0, premodulated=premod_in, next_styles=s1, only_next=True,
+                               **layer_kwargs)
                 pre = True
-            x, x_rgb = self.conv1(x, w1, fused_modconv=False, styles=s1, dcoefs=d1, premodulated=pre, next_styles=s_rgb, **layer_kwargs)
-            rgb_in = (x_rgb, s_rgb)
+            # ToRGB of <= 4 channels inside conv1's epilogue: a 3 x C dot product per pixel instead of x * s_rgb + a 1x1 convolution
+            fold_rgb = x.is_cuda and self.torgb.weight.shape[0] <= 4 and self.can_fold()
+            fold = {}
+            if x_next_styles is not None:
+                fold['y_styles'] = x_next_styles
+            if drop_x:
+                fold['emit_y'] = False
+            if fold_rgb:
+                fold['rgb'] = (self.torgb.weight, s_rgb, self.torgb.bias)
+            outs = self.conv1(x, w1, fused_modconv=False, styles=s1, dcoefs=d1, premodulated=pre, next_styles=None if fold_rgb else s_rgb,
+                              **fold, **layer_kwargs)          # (y | y * y_styles)?, (y * s_rgb | ToRGB output)
+            x = None if drop_x else outs[0]
+            if fold_rgb:
+                y_rgb = outs[-1]
+            else:
+                rgb_in = (outs[-1], s_rgb)
         else:
             if self.in_channels != 0:
                 x = self.conv0(x, w0, fused_modconv=fused_modconv, **layer_kwargs)
             x = self.conv1(x, w1, fused_modconv=fused_modconv, **layer_kwargs)
-        return x, w_rgb, fused_modconv, rgb_in
+        return x, w_rgb, fused_modconv, rgb_in, y_rgb
 
     def _torgb(self, x, w_rgb, fused_modconv, rgb_in, raw=False):
         if rgb_in is not None:
@@ -382,7 +423,9 @@ class SynthesisBlock(torch.nn.Module):
         return img.add_(y) if img is not None else y
 
     def forward(self, x, img, ws, force_fp32=False, fused_modconv=None, **layer_kwargs):
-        x, w_rgb, fused_modconv, rgb_in = self._features(x, ws, force_fp32, fused_modconv, layer_kwargs)
+        x, w_rgb, fused_modconv, rgb_in, y_rgb = self._features(x, ws, force_fp32, fused_modconv, layer_kwargs)
+        if y_rgb is not None:
+            return x, self._accumulate(img, y_rgb)
         if self._fuse_skip(rgb_in, img):
             y = self._torgb(x, w_rgb, fused_modconv, rgb_in, raw=True)
             return x, upfirdn2d.upsample2d_add(img, self.resample_filter, y, self.torgb.bias)
@@ -422,7 +465,9 @@ class SegSynthesisBlock(SynthesisBlock):
         return super()._load_from_state_dict(state_dict, prefix, *args, **kwargs)
 
     def forward(self, x, img, ws, condition_img=None, force_fp32=False, fused_modconv=None, **layer_kwargs):
-        x, w_shared, fused_modconv, rgb_in = self._features(x, ws, force_fp32, fused_modconv, layer_kwargs)
+        x, w_shared, fused_modconv, rgb_in, y = self._features(x, ws, force_fp32, fused_modconv, layer_kwargs)
+        if y is not None:
+            return x, self._accumulate(img, y[:, :self.img_channels]), self._accumulate(condition_img, y[:, self.img_channels:])
         if self._fuse_skip(rgb_in, img, condition_img):
             y, b, ci = self._torgb(x, w_shared, fused_modconv, rgb_in, raw=True), self.torgb.bias, self.img_channels
             img = upfirdn2d.upsample2d_add(img, self.resample_filter, y[:, :ci], b[:ci])

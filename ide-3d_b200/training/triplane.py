@@ -234,10 +234,29 @@ class SynthesisNetwork(torch.nn.Module):
             plan = _STYLE_PLANS[self] = networks.StylePlan(pairs)
         return plan.run(ws)
 
+    def _chain_kwargs(self, blocks, block_kwargs):
+        """Per-block keyword arguments that link consecutive blocks of one call (networks.FUSED_TORGB): every block but the last
+        returns `x * styles` of the next block's conv0 (its only consumer) instead of x, the next block takes that as premodulated
+        input, and the last block returns no x.  Needs the chained inference path in every block, which the style plan implies
+        unless fused_modconv is forced; otherwise the blocks run unlinked."""
+        plan = block_kwargs.get('style_plan')
+        if plan is None or block_kwargs.get('fused_modconv') or not all(b.can_fold() for b in blocks):
+            return [block_kwargs] * len(blocks)
+        out = []
+        for i, b in enumerate(blocks):
+            kw = dict(block_kwargs, premodulated_x=i > 0 and b.in_channels != 0)
+            if i + 1 < len(blocks):
+                kw['x_next_styles'] = plan[blocks[i + 1].conv0][0]
+            else:
+                kw['drop_x'] = True
+            out.append(kw)
+        return out
+
     def backbone(self, voxel_ws, **block_kwargs):
         x = img_v = seg_v = None
-        for res, cur_ws in zip(self.voxel_block_resolutions, voxel_ws):
-            x, img_v, seg_v = getattr(self, f'vb{res}')(x, img_v, cur_ws, condition_img=seg_v, **block_kwargs)
+        blocks = [getattr(self, f'vb{res}') for res in self.voxel_block_resolutions]
+        for block, cur_ws, kw in zip(blocks, voxel_ws, self._chain_kwargs(blocks, block_kwargs)):
+            x, img_v, seg_v = block(x, img_v, cur_ws, condition_img=seg_v, **kw)
         return img_v, seg_v
 
     def superres(self, feat_img, block_ws, **block_kwargs):
@@ -247,8 +266,9 @@ class SynthesisNetwork(torch.nn.Module):
             x = torch.nn.functional.interpolate(x, size=size, mode='bilinear', align_corners=False)
             rgb = torch.nn.functional.interpolate(rgb, size=size, mode='bilinear', align_corners=False)
         rgb = rgb.contiguous()
-        for res, cur_ws in zip(self.block_resolutions, block_ws):
-            x, rgb = getattr(self, f'b{res}')(x, rgb, cur_ws, **block_kwargs)
+        blocks = [getattr(self, f'b{res}') for res in self.block_resolutions]
+        for block, cur_ws, kw in zip(blocks, block_ws, self._chain_kwargs(blocks, block_kwargs)):
+            x, rgb = block(x, rgb, cur_ws, **kw)
         return rgb
 
     def forward(self, ws, c=None, render_params=None, noise_mode='const', force_fp32=False, return_seg=False,

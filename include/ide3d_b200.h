@@ -6,6 +6,7 @@
  *
  *   ide3d_bias_act            torch_utils/ops/bias_act.cpp:32       (params: bias_act.h:12-31)
  *   ide3d_modconv_epilogue    torch_utils/ops/fma.py:15 + bias_act.cpp:32 fused (extension; inversion/networks.py:104-105,512)
+ *   ide3d_modconv_epilogue_rgb  the same, plus the next `x * styles` and the block's ToRGB 1x1 convolution (extension; :100, :700-707)
  *   ide3d_upfirdn2d           torch_utils/ops/upfirdn2d.cpp:16      (params: upfirdn2d.h:14-40)
  *   ide3d_upfirdn2d_add       upfirdn2d + the skip-connection add (extension; inversion/networks.py:841-844)
  *   ide3d_upfirdn2d_epilogue  upfirdn2d + demodulation/noise/bias_act tail (extension; inversion/networks.py:104-105,512)
@@ -92,6 +93,20 @@ int ide3d_modconv_epilogue(const void* x, const void* scale, const void* noise, 
                            const void* scale2, void* y2, int dtype, int act, float alpha, float gain, float clamp,
                            int64_t n, int64_t c, int64_t hw, int64_t noise_batch, int channels_last,
                            ide3d_stream_t stream);
+
+/* Extension: the same epilogue (channels_last, float32) with the layers that consume it folded into the pass.
+ * t = bias_act(x * scale[n,c] + noise[(n),h,w], b[c], act, alpha, gain, clamp) as above, then any subset of
+ *     y   = t * yscale[n,c]  (yscale NULL: y = t)      e.g. the next block's `x * styles` of its first convolution
+ *     y2  = t * scale2[n,c]                             as ide3d_modconv_epilogue
+ *     rgb[n, o, h*w] = sum_c wrgb[o,c] * srgb[n,c] * t[n,h*w,c] + brgb[o]   for o < rgb_channels (1..4), dense NCHW:
+ *         the block's ToRGB layer (modulated 1x1 convolution without demodulation, inversion/networks.py:700-707)
+ * x, y, y2: [n, h*w, c]; scale, yscale, scale2, srgb [n*c]; wrgb [rgb_channels * c]; b [c]; brgb [rgb_channels] (may be NULL).
+ * Each pixel's rgb sum runs in a fixed order without atomics (bit-identical reruns).  Forward only.
+ * IDE3D_UNSUPPORTED unless dtype is IDE3D_F32, c % 4 == 0 and c <= 512. */
+int ide3d_modconv_epilogue_rgb(const void* x, const void* scale, const void* noise, const void* b, const void* yscale,
+                               void* y, const void* scale2, void* y2, const void* wrgb, const void* srgb, const void* brgb,
+                               void* rgb, int64_t rgb_channels, int dtype, int act, float alpha, float gain, float clamp,
+                               int64_t n, int64_t c, int64_t hw, int64_t noise_batch, ide3d_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * upfirdn2d: pad -> zero-upsample -> FIR -> decimate.  Field meaning = upfirdn2d_kernel_params
