@@ -147,6 +147,23 @@ class LpipsParams(C.Structure):
                 ('scratch', C.c_void_p), ('scratch_bytes', C.c_int64), ('grad_value', C.c_void_p)]
 
 
+SEG_STEM_MAX_CLASSES = 31                              # IDE3D_SEG_STEM_MAX_CLASSES
+
+
+class SegStemParams(C.Structure):
+    _fields_ = [('mask', C.c_void_p), ('n', C.c_int), ('h', C.c_int), ('w', C.c_int),
+                ('mask_stride_n', C.c_int64), ('mask_stride_h', C.c_int64), ('mask_stride_w', C.c_int64),
+                ('classes', C.c_int), ('c0', C.c_int), ('c1', C.c_int),
+                ('w0', C.c_void_p), ('b0', C.c_void_p), ('wg0', C.c_float), ('w1', C.c_void_p), ('b1', C.c_void_p), ('wg1', C.c_float),
+                ('ws', C.c_void_p), ('wgs', C.c_float), ('fir', C.c_void_p), ('tables', C.c_void_p), ('y1', C.c_void_p), ('skip', C.c_void_p)]
+
+
+class SegLabelsParams(C.Structure):
+    _fields_ = [('seg', C.c_void_p), ('n', C.c_int), ('classes', C.c_int), ('in_h', C.c_int), ('in_w', C.c_int),
+                ('seg_stride_n', C.c_int64), ('seg_stride_c', C.c_int64), ('seg_stride_h', C.c_int64), ('seg_stride_w', C.c_int64),
+                ('out_h', C.c_int), ('out_w', C.c_int), ('out', C.c_void_p)]
+
+
 _lib = None
 
 
@@ -232,10 +249,15 @@ def get_lib():
     lib.ide3d_lpips_scratch_bytes.restype = C.c_int64
     lib.ide3d_lpips_fwd.argtypes = [C.POINTER(LpipsParams), vp]
     lib.ide3d_lpips_bwd.argtypes = [C.POINTER(LpipsParams), vp]
+    lib.ide3d_seg_stem_scratch_bytes.argtypes = [i32, i32]
+    lib.ide3d_seg_stem_scratch_bytes.restype = C.c_int64
+    lib.ide3d_seg_stem.argtypes = [C.POINTER(SegStemParams), vp]
+    lib.ide3d_seg_labels.argtypes = [C.POINTER(SegLabelsParams), vp]
     for name in ('bias_act', 'upfirdn2d', 'filtered_lrelu', 'filtered_lrelu_act', 'raymarch_fwd', 'raymarch_bwd', 'raymarch_bwd_cam', 'sample_voxel',
                  'sigma_grid', 'planes_to_nhwc', 'initial_rays', 'transform_points', 'sample_triplane', 'integrate',
                  'sample_pdf', 'style_plan', 'mc_classify', 'mc_emit', 'mesh_normals', 'raster', 'video_frames', 'image_strips',
-                 'noise_reg', 'noise_normalize', 'seg_xent_fwd', 'seg_xent_bwd', 'lpips_fwd', 'lpips_bwd', 'abi_version'):
+                 'noise_reg', 'noise_normalize', 'seg_xent_fwd', 'seg_xent_bwd', 'lpips_fwd', 'lpips_bwd', 'seg_stem', 'seg_labels',
+                 'abi_version'):
         getattr(lib, 'ide3d_' + name).restype = C.c_int
     if lib.ide3d_abi_version() != 1:
         raise RuntimeError('ide3d_b200: ABI version mismatch between _lib.py and libide3d_b200.so')
@@ -252,7 +274,8 @@ def exported_symbols():
             'ide3d_sample_triplane', 'ide3d_integrate', 'ide3d_sample_pdf', 'ide3d_mask2color', 'ide3d_style_plan', 'ide3d_mc_classify', 'ide3d_mc_emit',
             'ide3d_mesh_normals', 'ide3d_raster_scratch_bytes', 'ide3d_raster', 'ide3d_video_frames', 'ide3d_image_strips',
             'ide3d_noise_reg', 'ide3d_noise_normalize', 'ide3d_seg_xent_fwd', 'ide3d_seg_xent_bwd',
-            'ide3d_lpips_scratch_bytes', 'ide3d_lpips_fwd', 'ide3d_lpips_bwd']
+            'ide3d_lpips_scratch_bytes', 'ide3d_lpips_fwd', 'ide3d_lpips_bwd', 'ide3d_seg_stem_scratch_bytes', 'ide3d_seg_stem',
+            'ide3d_seg_labels']
 
 
 def check(rc, allow_unsupported=False):

@@ -31,6 +31,9 @@
  *   ide3d_noise_normalize     inversion/training/projectors/w_projector_ide3d.py:138-142  noise renormalisation
  *   ide3d_seg_xent_fwd/_bwd   semantic-mask loss of the projector (extension): cross-entropy of the upsampled logits
  *   ide3d_lpips_fwd/_bwd      inversion/criteria/lpips/lpips.py:29-35 + utils.py:6-8  LPIPS head over all tapped layers (pivotal tuning)
+ *   ide3d_seg_stem            Painter/run_UI.py:290-295 + inversion/networks.py:1638-1646  one-hot mask -> stem, conv1 and skip of the
+ *                             HybridEncoder's geometry branch, from the class ids through per-class tables (extension)
+ *   ide3d_seg_labels          the generator's class ids at image resolution (extension; the starting mask of an edit)
  *
  * Conventions
  *   - plain C: raw device pointers, sizes, strides (in ELEMENTS), a cudaStream_t passed as void*.
@@ -553,6 +556,55 @@ typedef struct ide3d_lpips_params {
 int64_t ide3d_lpips_scratch_bytes(const ide3d_lpips_params* p);
 int ide3d_lpips_fwd(const ide3d_lpips_params* p, ide3d_stream_t stream);
 int ide3d_lpips_bwd(const ide3d_lpips_params* p, ide3d_stream_t stream);
+
+/* Opening of the HybridEncoder's geometry branch (inversion/networks.py:1638-1646) from a class-id mask (extension).  The branch's
+ * input one_hot(mask) * 2 - 1 takes `classes` + 1 distinct values per pixel (a mask value >= classes is the all-minus-one "no class"
+ * row, as mask2label_np makes it), so the 1x1 stem, block 0's 3x3 conv1 (bias, lrelu slope 0.2, gain sqrt 2, no clamp) and its
+ * [4, 4] FIR-down + 1x1 skip (no bias) become per-class tables:
+ *   T[k]     = wg0 (2 W0[:, k] - sum_j W0[:, j]) + b0     (no class: -wg0 sum_j W0[:, j] + b0)
+ *   y1[p]    = lrelu(b1 + sum_{taps t inside the image} wg1 W1[:, :, t] @ T[m(p + t)]) * sqrt 2
+ *   skip[q]  = sum_{4x4 taps a inside the image} f~[a] wgs Ws @ T[m(2q + a - 1)]        f~: f flipped, as upfirdn2d convolves
+ * The zero padding of conv1 and of the FIR pads the stem's OUTPUT: out-of-image taps contribute nothing.
+ * Two launches whatever n: one CTA builds the tables in double (fixed order) into `tables` (ide3d_seg_stem_scratch_bytes bytes,
+ * 16-byte aligned), then one CTA per 16 x 16 tile of y1 reads them from shared memory.  No atomics: reruns are bit-identical.
+ * mask uint8 [n, h, w], any element strides; w0 [c0, classes], w1 [c0, c0, 3, 3], ws [c1, c0], b0 / b1 [c0], fir [4, 4]: dense fp32.
+ * Outputs fp32 channels_last, dense: y1 [n, h, w, c0], skip [n, h / 2, w / 2, c1] (16-byte aligned, as are b1 and tables).
+ * IDE3D_UNSUPPORTED unless c0 is 32 or 64, c1 = 2 c0, classes <= IDE3D_SEG_STEM_MAX_CLASSES, h and w even and >= 8. */
+#define IDE3D_SEG_STEM_MAX_CLASSES 31
+typedef struct ide3d_seg_stem_params {
+    const uint8_t* mask;
+    int n, h, w;
+    int64_t mask_stride_n, mask_stride_h, mask_stride_w;
+    int classes, c0, c1;
+    const float* w0;
+    const float* b0;
+    float wg0;
+    const float* w1;
+    const float* b1;
+    float wg1;
+    const float* ws;
+    float wgs;
+    const float* fir;
+    float* tables;
+    float* y1;
+    float* skip;
+} ide3d_seg_stem_params;
+/* bytes of `tables` ide3d_seg_stem needs (IDE3D_UNSUPPORTED for a configuration it would refuse) */
+int64_t ide3d_seg_stem_scratch_bytes(int classes, int c0);
+int ide3d_seg_stem(const ide3d_seg_stem_params* p, ide3d_stream_t stream);
+
+/* Class ids of the generator's render at image resolution (extension): out[n, y, x] = argmax_k of the logits seg [n, classes, in_h,
+ * in_w] (fp32, any strides; the strided view G.synthesis(..., return_seg='raw') returns) upsampled bilinearly (align_corners=False)
+ * to out_h x out_w, with the rounding and tie rule of ide3d_video_frames / ide3d_image_strips.  out uint8 [n, out_h, out_w] dense.
+ * One launch; the upsampled logits are never built. */
+typedef struct ide3d_seg_labels_params {
+    const float* seg;
+    int n, classes, in_h, in_w;
+    int64_t seg_stride_n, seg_stride_c, seg_stride_h, seg_stride_w;
+    int out_h, out_w;
+    uint8_t* out;
+} ide3d_seg_labels_params;
+int ide3d_seg_labels(const ide3d_seg_labels_params* p, ide3d_stream_t stream);
 
 #ifdef __cplusplus
 }
