@@ -158,6 +158,12 @@ class SegStemParams(C.Structure):
                 ('ws', C.c_void_p), ('wgs', C.c_float), ('fir', C.c_void_p), ('tables', C.c_void_p), ('y1', C.c_void_p), ('skip', C.c_void_p)]
 
 
+class SegStemBwdParams(C.Structure):
+    _fields_ = [('fwd', SegStemParams), ('grad_y1', C.c_void_p), ('grad_skip', C.c_void_p), ('grad_w0', C.c_void_p),
+                ('grad_b0', C.c_void_p), ('grad_w1', C.c_void_p), ('grad_b1', C.c_void_p), ('grad_ws', C.c_void_p),
+                ('scratch', C.c_void_p), ('scratch_bytes', C.c_int64)]
+
+
 class SegLabelsParams(C.Structure):
     _fields_ = [('seg', C.c_void_p), ('n', C.c_int), ('classes', C.c_int), ('in_h', C.c_int), ('in_w', C.c_int),
                 ('seg_stride_n', C.c_int64), ('seg_stride_c', C.c_int64), ('seg_stride_h', C.c_int64), ('seg_stride_w', C.c_int64),
@@ -245,6 +251,8 @@ def get_lib():
     lib.ide3d_noise_normalize.argtypes = [C.POINTER(NoiseTable), vp]
     lib.ide3d_seg_xent_fwd.argtypes = [C.POINTER(SegXentParams), vp]
     lib.ide3d_seg_xent_bwd.argtypes = [C.POINTER(SegXentParams), vp]
+    lib.ide3d_seg_xent_fwd_ac.argtypes = [C.POINTER(SegXentParams), vp]
+    lib.ide3d_seg_xent_bwd_ac.argtypes = [C.POINTER(SegXentParams), vp]
     lib.ide3d_lpips_scratch_bytes.argtypes = [C.POINTER(LpipsParams)]
     lib.ide3d_lpips_scratch_bytes.restype = C.c_int64
     lib.ide3d_lpips_fwd.argtypes = [C.POINTER(LpipsParams), vp]
@@ -252,12 +260,16 @@ def get_lib():
     lib.ide3d_seg_stem_scratch_bytes.argtypes = [i32, i32]
     lib.ide3d_seg_stem_scratch_bytes.restype = C.c_int64
     lib.ide3d_seg_stem.argtypes = [C.POINTER(SegStemParams), vp]
+    lib.ide3d_seg_stem_bwd_scratch_bytes.argtypes = [i32, i32, i32, i32, i32]
+    lib.ide3d_seg_stem_bwd_scratch_bytes.restype = C.c_int64
+    lib.ide3d_seg_stem_bwd.argtypes = [C.POINTER(SegStemBwdParams), vp]
     lib.ide3d_seg_labels.argtypes = [C.POINTER(SegLabelsParams), vp]
+    lib.ide3d_seg_labels_ac.argtypes = [C.POINTER(SegLabelsParams), vp]
     for name in ('bias_act', 'upfirdn2d', 'filtered_lrelu', 'filtered_lrelu_act', 'raymarch_fwd', 'raymarch_bwd', 'raymarch_bwd_cam', 'sample_voxel',
                  'sigma_grid', 'planes_to_nhwc', 'initial_rays', 'transform_points', 'sample_triplane', 'integrate',
                  'sample_pdf', 'style_plan', 'mc_classify', 'mc_emit', 'mesh_normals', 'raster', 'video_frames', 'image_strips',
-                 'noise_reg', 'noise_normalize', 'seg_xent_fwd', 'seg_xent_bwd', 'lpips_fwd', 'lpips_bwd', 'seg_stem', 'seg_labels',
-                 'abi_version'):
+                 'noise_reg', 'noise_normalize', 'seg_xent_fwd', 'seg_xent_bwd', 'seg_xent_fwd_ac', 'seg_xent_bwd_ac', 'lpips_fwd',
+                 'lpips_bwd', 'seg_stem', 'seg_stem_bwd', 'seg_labels', 'seg_labels_ac', 'abi_version'):
         getattr(lib, 'ide3d_' + name).restype = C.c_int
     if lib.ide3d_abi_version() != 1:
         raise RuntimeError('ide3d_b200: ABI version mismatch between _lib.py and libide3d_b200.so')
@@ -275,7 +287,8 @@ def exported_symbols():
             'ide3d_mesh_normals', 'ide3d_raster_scratch_bytes', 'ide3d_raster', 'ide3d_video_frames', 'ide3d_image_strips',
             'ide3d_noise_reg', 'ide3d_noise_normalize', 'ide3d_seg_xent_fwd', 'ide3d_seg_xent_bwd',
             'ide3d_lpips_scratch_bytes', 'ide3d_lpips_fwd', 'ide3d_lpips_bwd', 'ide3d_seg_stem_scratch_bytes', 'ide3d_seg_stem',
-            'ide3d_seg_labels']
+            'ide3d_seg_labels', 'ide3d_seg_xent_fwd_ac', 'ide3d_seg_xent_bwd_ac', 'ide3d_seg_stem_bwd_scratch_bytes', 'ide3d_seg_stem_bwd',
+            'ide3d_seg_labels_ac']
 
 
 def check(rc, allow_unsupported=False):

@@ -3,7 +3,8 @@
 //                                            over the whole table of noise buffers in a fixed number of launches (the reference walks
 //                                            an avg-pool pyramid per buffer: a few hundred small torch kernels per step);
 //   ide3d_seg_xent_fwd / _bwd                the semantic-mask loss (extension): cross-entropy of the bilinearly upsampled logits,
-//                                            evaluated per output pixel from the render-resolution logits (seg_common.cuh).
+//                                            evaluated per output pixel from the render-resolution logits (seg_common.cuh);
+//                                            _fwd_ac / _bwd_ac are the same kernels with align_corners=True (BiSeNet's upsampling).
 // Every reduction runs in a fixed order (per-thread strides, then a shuffle / shared-memory tree): no float atomics, bit-reproducible.
 #include "seg_common.cuh"
 
@@ -179,7 +180,9 @@ static int noise_args(const ide3d_noise_table* t, bool need_scratch, NoiseArgs& 
 
 // ------------------------------------------------------------------------------------------------ semantic cross-entropy
 // Forward: one CTA per (output row, frame).  Per pixel: the bilinear logits (seg_logit_at), max, log-sum-exp, NLL of the mask class;
-// the row's NLL sum (double) goes to partials[frame * out_h + row] and one more CTA folds the partials in order.
+// the row's NLL sum (double) goes to partials[frame * out_h + row] and one more CTA folds the partials in order.  AC: the source
+// position rule (seg_common.cuh), align_corners=True for the _ac entry points.
+template <bool AC>
 __global__ void __launch_bounds__(kXentThreads) seg_xent_fwd_kernel(ide3d_seg_xent_params p) {
     __shared__ double red[33];
     const int y = blockIdx.x, n = blockIdx.y;
@@ -188,7 +191,7 @@ __global__ void __launch_bounds__(kXentThreads) seg_xent_fwd_kernel(ide3d_seg_xe
     float* lrow = p.lse + ((long long)n * p.out_h + y) * p.out_w;
     double acc = 0.0;
     for (int x = threadIdx.x; x < p.out_w; x += kXentThreads) {
-        const SegTaps t = seg_taps_at(s, p.in_h, p.in_w, p.seg_stride_h, p.seg_stride_w, x, y, p.out_h, p.out_w);
+        const SegTaps t = seg_taps_at<AC>(s, p.in_h, p.in_w, p.seg_stride_h, p.seg_stride_w, x, y, p.out_h, p.out_w);
         const int label = min((int)mrow[x], p.classes - 1);
         float mx = -INFINITY, vl = 0.f;
         for (int k = 0; k < p.classes; ++k) {
@@ -215,8 +218,17 @@ __global__ void __launch_bounds__(kNoiseThreads) seg_xent_loss_kernel(const doub
 }
 
 // First output index whose taps can reach source index i (lo) and one past the last (hi): a tap of output d reaches i0 = floor(src(d))
-// and i0 + 1, src(d) = (d + 0.5) * in / out - 0.5, so i0 in {i - 1, i}; one extra index each side absorbs the rounding of src.
+// and i0 + 1, so i0 in {i - 1, i}; one extra index each side absorbs the rounding of src.  align_corners=False: src(d) = (d + 0.5) *
+// in / out - 0.5; align_corners=True: src(d) = d * (in - 1) / (out - 1), and every output reads texel 0 when in = 1.
+template <bool AC>
 __device__ __forceinline__ void tap_window(int i, int in, int out, int& lo, int& hi) {
+    if (AC) {
+        if (in == 1) { lo = 0; hi = out; return; }
+        const double r = (double)(out - 1) / (in - 1);
+        lo = max(0, (int)floor((i - 1) * r) - 1);
+        hi = min(out, (int)ceil((i + 1) * r) + 2);
+        return;
+    }
     const double r = (double)out / in;
     lo = max(0, (int)floor((i - 0.5) * r - 0.5) - 1);
     hi = min(out, (int)ceil((i + 1.5) * r - 0.5) + 2);
@@ -224,6 +236,7 @@ __device__ __forceinline__ void tap_window(int i, int in, int out, int& lo, int&
 
 // Backward: one thread per (frame, class, source texel), ix fastest.  It visits the output pixels of its tap window and sums
 // w_y * w_x * (softmax_k - [mask == k]) in row order; softmax_k = exp(logit_k - lse) from the saved log-sum-exp.
+template <bool AC>
 __global__ void __launch_bounds__(kXentThreads) seg_xent_bwd_kernel(ide3d_seg_xent_params p, float scale) {
     const long long idx = (long long)blockIdx.x * kXentThreads + threadIdx.x;
     const long long total = (long long)p.n * p.classes * p.in_h * p.in_w;
@@ -233,21 +246,21 @@ __global__ void __launch_bounds__(kXentThreads) seg_xent_bwd_kernel(ide3d_seg_xe
     const float* s = p.seg + n * p.seg_stride_n;
     const long long kc = k * p.seg_stride_c;
     int y0, y1, x0, x1;
-    tap_window(iy, p.in_h, p.out_h, y0, y1);
-    tap_window(ix, p.in_w, p.out_w, x0, x1);
+    tap_window<AC>(iy, p.in_h, p.out_h, y0, y1);
+    tap_window<AC>(ix, p.in_w, p.out_w, x0, x1);
     const float g = scale * __ldg(p.grad_loss);
     float acc = 0.f;
     for (int y = y0; y < y1; ++y) {
-        const Tap ty = bilinear_tap(y, p.in_h, p.out_h);
+        const Tap ty = bilinear_tap<AC>(y, p.in_h, p.out_h);
         const float wy = (ty.i0 == iy ? ty.l0 : 0.f) + (ty.i1 == iy ? ty.l1 : 0.f);
         if (!(ty.i0 == iy || ty.i1 == iy)) continue;
         const long long row = ((long long)n * p.out_h + y) * p.out_w;
         float racc = 0.f;
         for (int x = x0; x < x1; ++x) {
-            const Tap tx = bilinear_tap(x, p.in_w, p.out_w);
+            const Tap tx = bilinear_tap<AC>(x, p.in_w, p.out_w);
             if (!(tx.i0 == ix || tx.i1 == ix)) continue;
             const float wx = (tx.i0 == ix ? tx.l0 : 0.f) + (tx.i1 == ix ? tx.l1 : 0.f);
-            const SegTaps t = seg_taps_at(s, p.in_h, p.in_w, p.seg_stride_h, p.seg_stride_w, x, y, p.out_h, p.out_w);
+            const SegTaps t = seg_taps_at<AC>(s, p.in_h, p.in_w, p.seg_stride_h, p.seg_stride_w, x, y, p.out_h, p.out_w);
             const float prob = expf(seg_logit_at(t, kc) - __ldg(p.lse + row + x));
             const float d = min((int)__ldg(p.mask + row + x), p.classes - 1) == k ? prob - 1.f : prob;
             racc += wx * d;
@@ -307,11 +320,12 @@ extern "C" int ide3d_noise_normalize(const ide3d_noise_table* t, ide3d_stream_t 
     return IDE3D_OK;
 }
 
-extern "C" int ide3d_seg_xent_fwd(const ide3d_seg_xent_params* p, ide3d_stream_t stream) {
+template <bool AC>
+static int seg_xent_fwd(const ide3d_seg_xent_params* p, ide3d_stream_t stream) {
     const int rc = ide3d::check_xent(p);
     if (rc != IDE3D_OK) return rc;
     IDE3D_REQUIRE(p->partials && p->loss, "seg_xent_fwd: null partials or loss");
-    ide3d::seg_xent_fwd_kernel<<<dim3((unsigned)p->out_h, (unsigned)p->n), ide3d::kXentThreads, 0, (cudaStream_t)stream>>>(*p);
+    ide3d::seg_xent_fwd_kernel<AC><<<dim3((unsigned)p->out_h, (unsigned)p->n), ide3d::kXentThreads, 0, (cudaStream_t)stream>>>(*p);
     IDE3D_CHECK_LAUNCH("seg_xent_fwd_kernel");
     ide3d::seg_xent_loss_kernel<<<1, ide3d::kNoiseThreads, 0, (cudaStream_t)stream>>>(p->partials, p->n * p->out_h,
                                                                                       (double)p->n * p->out_h * p->out_w, p->loss);
@@ -319,14 +333,20 @@ extern "C" int ide3d_seg_xent_fwd(const ide3d_seg_xent_params* p, ide3d_stream_t
     return IDE3D_OK;
 }
 
-extern "C" int ide3d_seg_xent_bwd(const ide3d_seg_xent_params* p, ide3d_stream_t stream) {
+template <bool AC>
+static int seg_xent_bwd(const ide3d_seg_xent_params* p, ide3d_stream_t stream) {
     const int rc = ide3d::check_xent(p);
     if (rc != IDE3D_OK) return rc;
     IDE3D_REQUIRE(p->grad_loss && p->grad_seg, "seg_xent_bwd: null grad_loss or grad_seg");
     const long long total = (long long)p->n * p->classes * p->in_h * p->in_w;
     const float scale = (float)(1.0 / ((double)p->n * p->out_h * p->out_w));
-    ide3d::seg_xent_bwd_kernel<<<(unsigned)ide3d::ceil_div(total, (long long)ide3d::kXentThreads), ide3d::kXentThreads, 0,
-                                 (cudaStream_t)stream>>>(*p, scale);
+    ide3d::seg_xent_bwd_kernel<AC><<<(unsigned)ide3d::ceil_div(total, (long long)ide3d::kXentThreads), ide3d::kXentThreads, 0,
+                                     (cudaStream_t)stream>>>(*p, scale);
     IDE3D_CHECK_LAUNCH("seg_xent_bwd_kernel");
     return IDE3D_OK;
 }
+
+extern "C" int ide3d_seg_xent_fwd(const ide3d_seg_xent_params* p, ide3d_stream_t stream) { return seg_xent_fwd<false>(p, stream); }
+extern "C" int ide3d_seg_xent_bwd(const ide3d_seg_xent_params* p, ide3d_stream_t stream) { return seg_xent_bwd<false>(p, stream); }
+extern "C" int ide3d_seg_xent_fwd_ac(const ide3d_seg_xent_params* p, ide3d_stream_t stream) { return seg_xent_fwd<true>(p, stream); }
+extern "C" int ide3d_seg_xent_bwd_ac(const ide3d_seg_xent_params* p, ide3d_stream_t stream) { return seg_xent_bwd<true>(p, stream); }

@@ -13,8 +13,10 @@ loads unchanged.  Activations are fp32 channels_last on the GPU, like training/n
 Extension: the semantic input may be a uint8 class-id mask [N, H, W] instead of the float map.  It stands for mask2label_np(mask)*2-1
 (dnnlib/seg_tools.py:67-72, Painter/run_UI.py:290-295): a value >= input_seg_dim is an all-zero one-hot row, i.e. -1 in every channel.
 The geometry branch then opens with ide3d_seg_stem (torch_utils/ops/seg_stem.py): the stem, block 0's conv1 and its skip computed from
-one byte per pixel through per-class tables, without building the one-hot map.  Shapes the kernel does not take, and calls that need
-gradients of those three layers, run the composition (device one-hot, *2-1, the three layers) instead.
+one byte per pixel through per-class tables, without building the one-hot map; under autograd its backward is ide3d_seg_stem_bwd,
+which gives those three layers' weight and bias gradients from the same tables.  Shapes the kernel does not take run the composition
+(device one-hot, *2-1, the three layers) instead, with or without gradients.  geometry(mask, signed=False) reads the mask as the
+{0, 1} one-hot instead (dnnlib/seg_tools.py:93-98 scatter, what encoder fine-tuning's cycle term feeds the encoder).
 """
 
 import math
@@ -116,6 +118,15 @@ def one_hot_input(mask, classes, dtype=torch.float32):
     return hot.permute(0, 3, 1, 2).to(dtype) * 2 - 1
 
 
+class _UnsignedStem:
+    """The stem's weight and bias re-parameterised for a {0, 1} one-hot input (see HybridEncoder._mask_stem); differentiable."""
+
+    def __init__(self, stem):
+        self.weight = stem.weight / 2
+        self.bias = stem.bias + stem.weight_gain / 2 * stem.weight.sum((1, 2, 3))
+        self.weight_gain = stem.weight_gain
+
+
 @persistence.persistent_class
 class HybridEncoder(torch.nn.Module):
     def __init__(self, size, n_latents_app, n_latents_geo, w_dim=512, add_dim=0, input_img_dim=3, input_seg_dim=19, **unused):
@@ -136,26 +147,29 @@ class HybridEncoder(torch.nn.Module):
         pws, pcm = out[:, :-self.add_dim], out[:, -self.add_dim:]
         return pws.reshape(len(img), self.n_latents_app, self.w_dim), pcm.reshape(len(img), self.add_dim)
 
-    def geometry(self, seg):
+    def geometry(self, seg, *, signed=True):
         """seg: the float semantic map [N, input_seg_dim, H, W] (one_hot * 2 - 1 or anything else), or a uint8 class-id mask [N, H, W]
-        -> [N, n_latents_geo, w_dim]."""
+        -> [N, n_latents_geo, w_dim].  A uint8 mask stands for one_hot * 2 - 1 (signed=True) or for the {0, 1} one_hot itself
+        (signed=False); a float map is used as it is."""
         if seg.dtype == torch.uint8:
             if seg.ndim != 3:
                 raise ValueError(f'HybridEncoder.geometry: a uint8 mask must be [N, H, W], got {tuple(seg.shape)}')
-            x = self._mask_stem(seg)
+            x = self._mask_stem(seg, signed)
             rest = self.convs_seg[2:]
         else:
             x, rest = _layout(seg), self.convs_seg
         return self.projector_seg(rest(x)).reshape(len(seg), self.n_latents_geo, self.w_dim)
 
-    def _mask_stem(self, mask):
-        """convs_seg[0:2] applied to one_hot_input(mask): the table kernel, or the composition it replaces."""
+    def _mask_stem(self, mask, signed=True):
+        """convs_seg[0:2] applied to one_hot_input(mask) (or its {0, 1} form): the table kernel, or the composition it replaces.
+        The kernel always reads one_hot * 2 - 1; for {0, 1} the stem is re-parameterised in front of it: with w0' = w0 / 2 and
+        b0' = b0 + wg0 / 2 * sum_j w0[:, j], wg0 w0' (2 h - 1) + b0' = wg0 w0 h + b0 (exact; the "no class" row gives b0)."""
         stem, block = self.convs_seg[0], self.convs_seg[1]
-        layers = (stem, block.conv1, block.skip)
-        need_grad = torch.is_grad_enabled() and any(p.requires_grad for m in layers for p in m.parameters())
-        out = None if need_grad else seg_stem.seg_stem(mask, stem, block.conv1, block.skip)
+        table_stem = stem if signed else _UnsignedStem(stem)
+        out = seg_stem.seg_stem(mask, table_stem, block.conv1, block.skip)
         if out is None:
-            return block(stem(_layout(one_hot_input(mask, self.input_seg_dim, stem.weight.dtype))))
+            x = one_hot_input(mask, self.input_seg_dim, stem.weight.dtype)
+            return block(stem(_layout(x if signed else (x + 1) / 2)))
         return block.tail(*out)
 
     def forward(self, img, seg):

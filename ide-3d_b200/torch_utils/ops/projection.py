@@ -3,8 +3,9 @@
     noise_regularizer(buffers)      the noise regulariser of inversion/training/projectors/w_projector_ide3d.py:113-122, one scalar
                                     over all buffers; ide3d_noise_reg computes it and, in the backward, every buffer's gradient
     noise_normalize_(buffers)       the renormalisation after each optimiser step (:138-142), in place (ide3d_noise_normalize)
-    seg_cross_entropy(seg_raw, mask) F.cross_entropy(upsample_seg(seg_raw, mask.shape[-2:]), mask) without the upsampled logits
-                                    (ide3d_seg_xent_fwd / _bwd)
+    seg_cross_entropy(seg_raw, mask, align_corners=False)   F.cross_entropy(upsample_seg(seg_raw, mask.shape[-2:]), mask) without
+                                    the upsampled logits (ide3d_seg_xent_fwd / _bwd); align_corners=True upsamples as BiSeNet does
+                                    (ide3d_seg_xent_fwd_ac / _bwd_ac), for encoder fine-tuning
 
 A buffer table the kernels have no specialisation for (a side that is not a power of two up to 512, more than 64 buffers -- the
 library answers IDE3D_UNSUPPORTED -- or a buffer that is not a dense fp32 square) runs the reference's torch loop instead.  CUDA
@@ -132,15 +133,17 @@ def _xent_params(seg_raw, mask, lse):
 
 class _SegXent(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, seg_raw, mask):
+    def forward(ctx, seg_raw, mask, align_corners):
         n, h, w = mask.shape
         lse = torch.empty([n, h, w], dtype=torch.float32, device=seg_raw.device)
         partials = torch.empty(n * h, dtype=torch.float64, device=seg_raw.device)
         loss = torch.empty(1, dtype=torch.float32, device=seg_raw.device)
         p = _xent_params(seg_raw, mask, lse)
         p.partials, p.loss = partials.data_ptr(), loss.data_ptr()
-        L.check(L.get_lib().ide3d_seg_xent_fwd(C.byref(p), L.stream_ptr(seg_raw.device)))
+        lib = L.get_lib()
+        L.check((lib.ide3d_seg_xent_fwd_ac if align_corners else lib.ide3d_seg_xent_fwd)(C.byref(p), L.stream_ptr(seg_raw.device)))
         ctx.save_for_backward(seg_raw, mask, lse)
+        ctx.align_corners = align_corners
         return loss.reshape(())
 
     @staticmethod
@@ -150,12 +153,13 @@ class _SegXent(torch.autograd.Function):
         g = grad_output.detach().reshape(1).to(torch.float32).contiguous()
         p = _xent_params(seg_raw, mask, lse)
         p.grad_loss, p.grad_seg = g.data_ptr(), grad.data_ptr()
-        L.check(L.get_lib().ide3d_seg_xent_bwd(C.byref(p), L.stream_ptr(seg_raw.device)))
-        return grad, None
+        lib = L.get_lib()
+        L.check((lib.ide3d_seg_xent_bwd_ac if ctx.align_corners else lib.ide3d_seg_xent_bwd)(C.byref(p), L.stream_ptr(seg_raw.device)))
+        return grad, None, None
 
 
-def seg_cross_entropy(seg_raw, mask):
-    """F.cross_entropy(interpolate(seg_raw, mask.shape[-2:], mode='bilinear', align_corners=False), mask.long()), mean reduction.
+def seg_cross_entropy(seg_raw, mask, align_corners=False):
+    """F.cross_entropy(interpolate(seg_raw, mask.shape[-2:], mode='bilinear', align_corners=align_corners), mask.long()), mean reduction.
     seg_raw float32 [N, C, R, R'] with C <= 32, any strides (the return_seg='raw' view of G.synthesis); mask uint8 [N, H, W] with
     values < C.  The values are not checked here (that would synchronise every call; the projector validates its mask once): the
     kernels read a label >= C as C - 1, where F.cross_entropy would raise."""
@@ -164,4 +168,4 @@ def seg_cross_entropy(seg_raw, mask):
         raise RuntimeError(f'seg_cross_entropy: seg_raw must be float32 [N, C <= 32, R, R], got {seg_raw.dtype} {tuple(seg_raw.shape)}')
     if mask.dtype != torch.uint8 or mask.ndim != 3 or mask.shape[0] != seg_raw.shape[0]:
         raise RuntimeError(f'seg_cross_entropy: mask must be uint8 [{seg_raw.shape[0]}, H, W], got {mask.dtype} {tuple(mask.shape)}')
-    return _SegXent.apply(seg_raw, mask.contiguous())
+    return _SegXent.apply(seg_raw, mask.contiguous(), bool(align_corners))

@@ -30,10 +30,13 @@
  *   ide3d_noise_reg           inversion/training/projectors/w_projector_ide3d.py:113-122  noise regulariser (+ its gradient)
  *   ide3d_noise_normalize     inversion/training/projectors/w_projector_ide3d.py:138-142  noise renormalisation
  *   ide3d_seg_xent_fwd/_bwd   semantic-mask loss of the projector (extension): cross-entropy of the upsampled logits
+ *   ide3d_seg_xent_*_ac       apps/finetune_hybrid_encoder.py:171-174  the same with align_corners=True (BiSeNet's upsampling)
  *   ide3d_lpips_fwd/_bwd      inversion/criteria/lpips/lpips.py:29-35 + utils.py:6-8  LPIPS head over all tapped layers (pivotal tuning)
  *   ide3d_seg_stem            Painter/run_UI.py:290-295 + inversion/networks.py:1638-1646  one-hot mask -> stem, conv1 and skip of the
  *                             HybridEncoder's geometry branch, from the class ids through per-class tables (extension)
+ *   ide3d_seg_stem_bwd        its gradients w.r.t. the three layers' weights (encoder fine-tuning)
  *   ide3d_seg_labels          the generator's class ids at image resolution (extension; the starting mask of an edit)
+ *   ide3d_seg_labels_ac       dnnlib/seg_tools.py:101-117  argmax of BiSeNet's align_corners=True upsampling
  *
  * Conventions
  *   - plain C: raw device pointers, sizes, strides (in ELEMENTS), a cudaStream_t passed as void*.
@@ -514,6 +517,10 @@ typedef struct ide3d_seg_xent_params {
 } ide3d_seg_xent_params;
 int ide3d_seg_xent_fwd(const ide3d_seg_xent_params* p, ide3d_stream_t stream);
 int ide3d_seg_xent_bwd(const ide3d_seg_xent_params* p, ide3d_stream_t stream);
+/* The same pair with align_corners=True (source position d * (in - 1) / (out - 1)), same parameters and limits: the cross-entropy of
+ * BiSeNet's upsampled logits (inversion/BiSeNet.py:249) for encoder fine-tuning. */
+int ide3d_seg_xent_fwd_ac(const ide3d_seg_xent_params* p, ide3d_stream_t stream);
+int ide3d_seg_xent_bwd_ac(const ide3d_seg_xent_params* p, ide3d_stream_t stream);
 
 /* LPIPS v0.1 head of pivotal tuning (inversion/criteria/lpips/{lpips,utils}.py, the pip `lpips` package) over every tapped layer of
  * one call.  Per layer l, sample n and pixel p, with the norm over the channels:
@@ -593,6 +600,32 @@ typedef struct ide3d_seg_stem_params {
 int64_t ide3d_seg_stem_scratch_bytes(int classes, int c0);
 int ide3d_seg_stem(const ide3d_seg_stem_params* p, ide3d_stream_t stream);
 
+/* Backward of ide3d_seg_stem: the gradients of w0, b0, w1, b1 and ws from grad_y1 [n, h, w, c0] and grad_skip [n, h / 2, w / 2, c1]
+ * (fp32 channels_last, dense; grad_y1 16-byte aligned).  `fwd` is the forward's parameter block with its tables already built (the
+ * lrelu's derivative is taken at the pre-activation recomputed from them).  Outputs dense fp32, overwritten: grad_w0 [c0, classes],
+ * grad_b0 [c0], grad_w1 [c0, c0, 3, 3], grad_b1 [c0], grad_ws [c1, c0].
+ *   launch 1: a fixed grid of CTAs sums the per-class gradients of the conv1 and skip tables over fixed sets of 16 x 16 tiles, each
+ *             bin column owned by one thread walking its tile in order, into per-CTA slices of `scratch`;
+ *   launch 2: the slices are folded in block order, in double;
+ *   launch 3: one CTA runs the chain to the parameters in double in a fixed order (the mirror of the forward's table launch).
+ * Three launches whatever n, no float atomics: reruns are bit-identical.  scratch: ide3d_seg_stem_bwd_scratch_bytes bytes, 16-byte
+ * aligned.  Limits are the forward's (IDE3D_UNSUPPORTED otherwise); everything is validated before the device is touched. */
+typedef struct ide3d_seg_stem_bwd_params {
+    ide3d_seg_stem_params fwd;
+    const float* grad_y1;
+    const float* grad_skip;
+    float* grad_w0;
+    float* grad_b0;
+    float* grad_w1;
+    float* grad_b1;
+    float* grad_ws;
+    void* scratch;
+    int64_t scratch_bytes;
+} ide3d_seg_stem_bwd_params;
+/* bytes of `scratch` ide3d_seg_stem_bwd needs (IDE3D_UNSUPPORTED for a shape the forward refuses, IDE3D_INVALID for bad sizes) */
+int64_t ide3d_seg_stem_bwd_scratch_bytes(int n, int h, int w, int classes, int c0);
+int ide3d_seg_stem_bwd(const ide3d_seg_stem_bwd_params* p, ide3d_stream_t stream);
+
 /* Class ids of the generator's render at image resolution (extension): out[n, y, x] = argmax_k of the logits seg [n, classes, in_h,
  * in_w] (fp32, any strides; the strided view G.synthesis(..., return_seg='raw') returns) upsampled bilinearly (align_corners=False)
  * to out_h x out_w, with the rounding and tie rule of ide3d_video_frames / ide3d_image_strips.  out uint8 [n, out_h, out_w] dense.
@@ -605,6 +638,8 @@ typedef struct ide3d_seg_labels_params {
     uint8_t* out;
 } ide3d_seg_labels_params;
 int ide3d_seg_labels(const ide3d_seg_labels_params* p, ide3d_stream_t stream);
+/* The same with align_corners=True (source position d * (in - 1) / (out - 1)): BiSeNet's upsampling (inversion/BiSeNet.py:249). */
+int ide3d_seg_labels_ac(const ide3d_seg_labels_params* p, ide3d_stream_t stream);
 
 #ifdef __cplusplus
 }
