@@ -147,6 +147,19 @@ class LpipsParams(C.Structure):
                 ('scratch', C.c_void_p), ('scratch_bytes', C.c_int64), ('grad_value', C.c_void_p)]
 
 
+FEAT_L1_MAX_LAYERS = 8                                 # IDE3D_FEAT_L1_MAX_LAYERS
+
+
+class FeatL1Layer(C.Structure):
+    _fields_ = [('c', C.c_int), ('h', C.c_int), ('w', C.c_int), ('weight', C.c_float), ('x', C.c_void_p), ('x_stride', C.c_int64 * 4),
+                ('y', C.c_void_p), ('y_stride', C.c_int64 * 4), ('grad_x', C.c_void_p), ('gx_stride', C.c_int64 * 4)]
+
+
+class FeatL1Params(C.Structure):
+    _fields_ = [('n', C.c_int), ('num_layers', C.c_int), ('dtype', C.c_int), ('layers', FeatL1Layer * FEAT_L1_MAX_LAYERS),
+                ('value', C.c_void_p), ('scratch', C.c_void_p), ('scratch_bytes', C.c_int64), ('grad_value', C.c_void_p)]
+
+
 SEG_STEM_MAX_CLASSES = 31                              # IDE3D_SEG_STEM_MAX_CLASSES
 
 
@@ -257,6 +270,10 @@ def get_lib():
     lib.ide3d_lpips_scratch_bytes.restype = C.c_int64
     lib.ide3d_lpips_fwd.argtypes = [C.POINTER(LpipsParams), vp]
     lib.ide3d_lpips_bwd.argtypes = [C.POINTER(LpipsParams), vp]
+    lib.ide3d_feat_l1_scratch_bytes.argtypes = [C.POINTER(FeatL1Params)]
+    lib.ide3d_feat_l1_scratch_bytes.restype = C.c_int64
+    lib.ide3d_feat_l1_fwd.argtypes = [C.POINTER(FeatL1Params), vp]
+    lib.ide3d_feat_l1_bwd.argtypes = [C.POINTER(FeatL1Params), vp]
     lib.ide3d_seg_stem_scratch_bytes.argtypes = [i32, i32]
     lib.ide3d_seg_stem_scratch_bytes.restype = C.c_int64
     lib.ide3d_seg_stem.argtypes = [C.POINTER(SegStemParams), vp]
@@ -269,7 +286,7 @@ def get_lib():
                  'sigma_grid', 'planes_to_nhwc', 'initial_rays', 'transform_points', 'sample_triplane', 'integrate',
                  'sample_pdf', 'style_plan', 'mc_classify', 'mc_emit', 'mesh_normals', 'raster', 'video_frames', 'image_strips',
                  'noise_reg', 'noise_normalize', 'seg_xent_fwd', 'seg_xent_bwd', 'seg_xent_fwd_ac', 'seg_xent_bwd_ac', 'lpips_fwd',
-                 'lpips_bwd', 'seg_stem', 'seg_stem_bwd', 'seg_labels', 'seg_labels_ac', 'abi_version'):
+                 'lpips_bwd', 'seg_stem', 'seg_stem_bwd', 'seg_labels', 'seg_labels_ac', 'feat_l1_fwd', 'feat_l1_bwd', 'abi_version'):
         getattr(lib, 'ide3d_' + name).restype = C.c_int
     if lib.ide3d_abi_version() != 1:
         raise RuntimeError('ide3d_b200: ABI version mismatch between _lib.py and libide3d_b200.so')
@@ -288,7 +305,7 @@ def exported_symbols():
             'ide3d_noise_reg', 'ide3d_noise_normalize', 'ide3d_seg_xent_fwd', 'ide3d_seg_xent_bwd',
             'ide3d_lpips_scratch_bytes', 'ide3d_lpips_fwd', 'ide3d_lpips_bwd', 'ide3d_seg_stem_scratch_bytes', 'ide3d_seg_stem',
             'ide3d_seg_labels', 'ide3d_seg_xent_fwd_ac', 'ide3d_seg_xent_bwd_ac', 'ide3d_seg_stem_bwd_scratch_bytes', 'ide3d_seg_stem_bwd',
-            'ide3d_seg_labels_ac']
+            'ide3d_seg_labels_ac', 'ide3d_feat_l1_scratch_bytes', 'ide3d_feat_l1_fwd', 'ide3d_feat_l1_bwd']
 
 
 def check(rc, allow_unsupported=False):

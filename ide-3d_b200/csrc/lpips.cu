@@ -185,7 +185,214 @@ static int lpips_args(const ide3d_lpips_params* p, bool backward, LpipsArgs& a, 
     return IDE3D_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------------------
+// The multi-tap L1 head of the encoder's VGG loss (apps/train_hybrid_encoder.py:143-152): total = sum_l w_l mean|x_l - y_l|.  The
+// same structure as the LPIPS head: one grid over every layer (a CTA finds its layer from its block index), partials in double, a
+// second launch that folds them in block order; the backward is one launch.  Work unit: one CTA per kFeatTile consecutive elements of
+// one layer.  A layer whose x, y (and grad_x) share one dense layout (NCHW or channels_last) is walked as a flat array, with float4
+// accesses when aligned; any other layer is walked in logical NCHW order through its strides.
+
+constexpr int kFeatVec = 4;
+constexpr int kFeatIters = 4;
+constexpr long long kFeatTile = (long long)kLpipsThreads * kFeatVec * kFeatIters;   // elements per CTA
+enum FeatMode { kFeatStrided = 0, kFeatFlat = 1, kFeatFlat4 = 2 };
+
+struct FeatL1Args {
+    ide3d_feat_l1_params p;
+    long long numel[IDE3D_FEAT_L1_MAX_LAYERS];
+    int mode[IDE3D_FEAT_L1_MAX_LAYERS];
+    int first_block[IDE3D_FEAT_L1_MAX_LAYERS + 1];
+    double* partials;                                // [grid]
+};
+
+__device__ __forceinline__ int feat_layer(const FeatL1Args& a) {
+    int l = 0;
+    while (l + 1 < a.p.num_layers && (int)blockIdx.x >= a.first_block[l + 1]) ++l;
+    return l;
+}
+
+// element offset of logical NCHW index e under strides s
+__device__ __forceinline__ long long feat_offset(const ide3d_feat_l1_layer& L, long long e, const int64_t* s) {
+    const long long w = e % L.w;
+    e /= L.w;
+    const long long h = e % L.h;
+    e /= L.h;
+    const long long c = e % L.c;
+    return (e / L.c) * s[0] + c * s[1] + h * s[2] + w * s[3];
+}
+
+__global__ void __launch_bounds__(kLpipsThreads) feat_l1_fwd_kernel(const __grid_constant__ FeatL1Args a) {
+    __shared__ double red[kLpipsThreads / 32];
+    const int l = feat_layer(a);
+    const ide3d_feat_l1_layer& L = a.p.layers[l];
+    const long long n = a.numel[l];
+    const long long base = (long long)(blockIdx.x - a.first_block[l]) * kFeatTile;
+    float acc = 0.f;
+    if (a.mode[l] == kFeatFlat4) {
+        const float4* x = reinterpret_cast<const float4*>(L.x);
+        const float4* y = reinterpret_cast<const float4*>(L.y);
+#pragma unroll
+        for (int it = 0; it < kFeatIters; ++it) {
+            const long long e = base + ((long long)it * kLpipsThreads + threadIdx.x) * kFeatVec;
+            if (e < n) {
+                const float4 u = __ldg(x + e / kFeatVec), v = __ldg(y + e / kFeatVec);
+                acc += fabsf(u.x - v.x) + fabsf(u.y - v.y) + fabsf(u.z - v.z) + fabsf(u.w - v.w);
+            }
+        }
+    } else {
+        for (int it = 0; it < kFeatIters * kFeatVec; ++it) {
+            const long long e = base + (long long)it * kLpipsThreads + threadIdx.x;
+            if (e < n) {
+                const long long ox = a.mode[l] == kFeatFlat ? e : feat_offset(L, e, L.x_stride);
+                const long long oy = a.mode[l] == kFeatFlat ? e : feat_offset(L, e, L.y_stride);
+                acc += fabsf(__ldg(L.x + ox) - __ldg(L.y + oy));
+            }
+        }
+    }
+    const double s = lpips_block_sum((double)acc, red);
+    if (threadIdx.x == 0) a.partials[blockIdx.x] = s;
+}
+
+// One CTA: per layer, thread t sums partials t, t + 256, ... in order, a fixed tree adds the threads; thread 0 adds the layers in order.
+__global__ void __launch_bounds__(kLpipsThreads) feat_l1_fold_kernel(const __grid_constant__ FeatL1Args a) {
+    __shared__ double red[kLpipsThreads / 32];
+    double total = 0.0;
+    for (int l = 0; l < a.p.num_layers; ++l) {
+        double s = 0.0;
+        for (int b = a.first_block[l] + threadIdx.x; b < a.first_block[l + 1]; b += kLpipsThreads) s += a.partials[b];
+        s = lpips_block_sum(s, red);
+        if (threadIdx.x == 0) {
+            const double mean = s / (double)a.numel[l];
+            a.p.value[l] = (float)mean;
+            total += (double)a.p.layers[l].weight * mean;
+        }
+        __syncthreads();                             // red is reused by the next layer
+    }
+    if (threadIdx.x == 0) a.p.value[a.p.num_layers] = (float)total;
+}
+
+__device__ __forceinline__ float feat_sgn(float d) { return (float)((d > 0.f) - (d < 0.f)); }
+
+// grad_x = g w_l / numel_l sgn(x - y), torch's sgn (0 where x == y); g read from device memory.
+__global__ void __launch_bounds__(kLpipsThreads) feat_l1_bwd_kernel(const __grid_constant__ FeatL1Args a) {
+    const int l = feat_layer(a);
+    const ide3d_feat_l1_layer& L = a.p.layers[l];
+    const long long n = a.numel[l];
+    const long long base = (long long)(blockIdx.x - a.first_block[l]) * kFeatTile;
+    const float gs = __ldg(a.p.grad_value) * (float)((double)L.weight / (double)n);
+    if (a.mode[l] == kFeatFlat4) {
+        const float4* x = reinterpret_cast<const float4*>(L.x);
+        const float4* y = reinterpret_cast<const float4*>(L.y);
+        float4* gx = reinterpret_cast<float4*>(L.grad_x);
+#pragma unroll
+        for (int it = 0; it < kFeatIters; ++it) {
+            const long long e = base + ((long long)it * kLpipsThreads + threadIdx.x) * kFeatVec;
+            if (e < n) {
+                const float4 u = __ldg(x + e / kFeatVec), v = __ldg(y + e / kFeatVec);
+                gx[e / kFeatVec] = make_float4(gs * feat_sgn(u.x - v.x), gs * feat_sgn(u.y - v.y), gs * feat_sgn(u.z - v.z),
+                                               gs * feat_sgn(u.w - v.w));
+            }
+        }
+    } else {
+        for (int it = 0; it < kFeatIters * kFeatVec; ++it) {
+            const long long e = base + (long long)it * kLpipsThreads + threadIdx.x;
+            if (e < n) {
+                const bool flat = a.mode[l] == kFeatFlat;
+                const long long ox = flat ? e : feat_offset(L, e, L.x_stride);
+                const long long oy = flat ? e : feat_offset(L, e, L.y_stride);
+                const long long og = flat ? e : feat_offset(L, e, L.gx_stride);
+                L.grad_x[og] = gs * feat_sgn(__ldg(L.x + ox) - __ldg(L.y + oy));
+            }
+        }
+    }
+}
+
+// True when strides s describe a dense, non-overlapping layout of [n, c, h, w] (size-1 dimensions ignored).
+static bool feat_dense(const int* size, const int64_t* s) {
+    int order[4] = {0, 1, 2, 3};
+    for (int i = 0; i < 4; ++i)                      // fastest dimension first
+        for (int j = i + 1; j < 4; ++j)
+            if (s[order[j]] < s[order[i]]) { const int t = order[i]; order[i] = order[j]; order[j] = t; }
+    long long expect = 1;
+    for (int i = 0; i < 4; ++i) {
+        const int d = order[i];
+        if (size[d] == 1) continue;
+        if (s[d] != expect) return false;
+        expect *= size[d];
+    }
+    return true;
+}
+
+static int feat_l1_args(const ide3d_feat_l1_params* p, bool backward, FeatL1Args& a) {
+    IDE3D_REQUIRE(p, "feat_l1: null params");
+    IDE3D_REQUIRE(p->n > 0 && p->num_layers > 0, "feat_l1: %d samples, %d layers", p->n, p->num_layers);
+    if (p->num_layers > IDE3D_FEAT_L1_MAX_LAYERS || p->dtype != IDE3D_F32) {
+        snprintf(error_buffer(), 512, "feat_l1: %d layers of dtype %d; the kernel takes at most %d fp32 layers", p->num_layers, p->dtype,
+                 IDE3D_FEAT_L1_MAX_LAYERS);
+        return IDE3D_UNSUPPORTED;
+    }
+    a.p = *p;
+    long long blocks = 0;
+    for (int l = 0; l < p->num_layers; ++l) {
+        const ide3d_feat_l1_layer& L = p->layers[l];
+        IDE3D_REQUIRE(L.c > 0 && L.h > 0 && L.w > 0, "feat_l1: layer %d has bad sizes (c %d, h %d, w %d)", l, L.c, L.h, L.w);
+        IDE3D_REQUIRE(L.x && L.y, "feat_l1: layer %d has a null x or y", l);
+        IDE3D_REQUIRE(!backward || L.grad_x, "feat_l1: layer %d has a null grad_x", l);
+        for (int k = 0; k < 4; ++k)
+            IDE3D_REQUIRE(L.x_stride[k] >= 0 && L.y_stride[k] >= 0 && (!backward || L.gx_stride[k] >= 0),
+                          "feat_l1: layer %d has a negative stride", l);
+        const int size[4] = {p->n, L.c, L.h, L.w};
+        a.numel[l] = (long long)p->n * L.c * L.h * L.w;
+        bool flat = feat_dense(size, L.x_stride);
+        for (int k = 0; k < 4; ++k) {
+            if (size[k] == 1) continue;
+            flat = flat && L.y_stride[k] == L.x_stride[k] && (!backward || L.gx_stride[k] == L.x_stride[k]);
+        }
+        const bool aligned = ((reinterpret_cast<uintptr_t>(L.x) | reinterpret_cast<uintptr_t>(L.y) |
+                               (backward ? reinterpret_cast<uintptr_t>(L.grad_x) : 0)) & 15) == 0;
+        a.mode[l] = !flat ? kFeatStrided : (aligned && a.numel[l] % kFeatVec == 0) ? kFeatFlat4 : kFeatFlat;
+        a.first_block[l] = (int)blocks;
+        blocks += ceil_div(a.numel[l], kFeatTile);
+        IDE3D_REQUIRE(blocks < (1LL << 31), "feat_l1: more than 2^31 blocks");
+    }
+    a.first_block[p->num_layers] = (int)blocks;
+    a.partials = nullptr;
+    return IDE3D_OK;
+}
+
 }  // namespace ide3d
+
+extern "C" int64_t ide3d_feat_l1_scratch_bytes(const ide3d_feat_l1_params* p) {
+    ide3d::FeatL1Args a;
+    const int rc = ide3d::feat_l1_args(p, false, a);
+    return rc != IDE3D_OK ? (int64_t)rc : (int64_t)8 * a.first_block[p->num_layers];
+}
+
+extern "C" int ide3d_feat_l1_fwd(const ide3d_feat_l1_params* p, ide3d_stream_t stream) {
+    ide3d::FeatL1Args a;
+    const int rc = ide3d::feat_l1_args(p, false, a);
+    if (rc != IDE3D_OK) return rc;
+    const long long grid = a.first_block[p->num_layers];
+    IDE3D_REQUIRE(p->value && p->scratch, "feat_l1_fwd: null value or scratch");
+    IDE3D_REQUIRE((reinterpret_cast<uintptr_t>(p->scratch) & 7) == 0, "feat_l1_fwd: scratch not 8-byte aligned");
+    IDE3D_REQUIRE(p->scratch_bytes >= 8 * grid, "feat_l1_fwd: scratch holds %lld bytes, need %lld", (long long)p->scratch_bytes, 8 * grid);
+    a.partials = static_cast<double*>(p->scratch);
+    ide3d::feat_l1_fwd_kernel<<<(unsigned)grid, ide3d::kLpipsThreads, 0, (cudaStream_t)stream>>>(a);
+    IDE3D_CHECK_LAUNCH("feat_l1_fwd_kernel");
+    ide3d::feat_l1_fold_kernel<<<1, ide3d::kLpipsThreads, 0, (cudaStream_t)stream>>>(a);
+    IDE3D_CHECK_LAUNCH("feat_l1_fold_kernel");
+    return IDE3D_OK;
+}
+
+extern "C" int ide3d_feat_l1_bwd(const ide3d_feat_l1_params* p, ide3d_stream_t stream) {
+    ide3d::FeatL1Args a;
+    const int rc = ide3d::feat_l1_args(p, true, a);
+    if (rc != IDE3D_OK) return rc;
+    IDE3D_REQUIRE(p->grad_value, "feat_l1_bwd: null grad_value");
+    ide3d::feat_l1_bwd_kernel<<<(unsigned)a.first_block[p->num_layers], ide3d::kLpipsThreads, 0, (cudaStream_t)stream>>>(a);
+    IDE3D_CHECK_LAUNCH("feat_l1_bwd_kernel");
+    return IDE3D_OK;
+}
 
 extern "C" int64_t ide3d_lpips_scratch_bytes(const ide3d_lpips_params* p) {
     ide3d::LpipsArgs a;

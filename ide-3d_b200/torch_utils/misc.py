@@ -1,9 +1,11 @@
-"""Small helpers with the reference's names (torch_utils/misc.py): assert_shape :48, profiled_function :100."""
+"""Small helpers with the reference's names (torch_utils/misc.py): assert_shape :48, profiled_function :100, InfiniteSampler :111."""
 
 import contextlib
 import functools
+import itertools
 import warnings
 
+import numpy as np
 import torch
 
 
@@ -31,3 +33,35 @@ def suppress_tracer_warnings():
         yield
     finally:
         warnings.filters.remove(flt)
+
+
+class InfiniteSampler(torch.utils.data.Sampler):
+    """Loops over the dataset forever (the reference's torch_utils/misc.py:111-145).  All ranks share one stream: a permutation drawn from
+    RandomState(seed), read cyclically, where each item read swaps its slot with one of the round(window_size * len) slots ending at it,
+    so the order drifts from lap to lap.  Rank r of num_replicas takes the stream's items r, r + num_replicas, ...: the shares are
+    disjoint.  With shuffle=False the stream is 0, 1, ..., len - 1 over and over."""
+
+    def __init__(self, dataset, rank=0, num_replicas=1, shuffle=True, seed=0, window_size=0.5):
+        if not (len(dataset) > 0 and num_replicas > 0 and 0 <= rank < num_replicas and 0 <= window_size <= 1):
+            raise ValueError(f'InfiniteSampler: {len(dataset)} items, rank {rank} of {num_replicas}, window {window_size}')
+        super().__init__()
+        self.dataset, self.rank, self.num_replicas = dataset, rank, num_replicas
+        self.shuffle, self.seed, self.window_size = shuffle, seed, window_size
+
+    def _stream(self):
+        n = len(self.dataset)
+        perm = np.arange(n)
+        if not self.shuffle:
+            yield from itertools.cycle(perm)
+        rng = np.random.RandomState(self.seed)
+        rng.shuffle(perm)
+        span = int(np.rint(n * self.window_size))
+        for slot in itertools.cycle(range(n)):
+            item = perm[slot]
+            if span > 1:
+                other = (slot - rng.randint(span)) % n
+                perm[[slot, other]] = perm[[other, slot]]
+            yield item
+
+    def __iter__(self):
+        return itertools.islice(self._stream(), self.rank, None, self.num_replicas)

@@ -143,13 +143,14 @@ def truncated_normal_(tensor, mean=0, std=1):
 
 
 def sample_camera_positions(device, n=1, r=1, horizontal_stddev=0.3, vertical_stddev=0.155,
-                            horizontal_mean=math.pi * 0.5, vertical_mean=math.pi * 0.5, mode='normal'):
-    """n camera origins on a sphere of radius r: theta = yaw, phi = pitch; returns (origins, phi, theta)."""
+                            horizontal_mean=math.pi * 0.5, vertical_mean=math.pi * 0.5, mode='normal', generator=None):
+    """n camera origins on a sphere of radius r: theta = yaw, phi = pitch; returns (origins, phi, theta).  `generator` (a
+    torch.Generator on `device`) feeds the uniform and gaussian draws instead of the global RNG."""
     def uni():
-        return torch.rand((n, 1), device=device) - 0.5
+        return torch.rand((n, 1), device=device, generator=generator) - 0.5
 
     def gau():
-        return torch.randn((n, 1), device=device)
+        return torch.randn((n, 1), device=device, generator=generator)
 
     if mode == 'uniform':
         theta = uni() * 2 * horizontal_stddev + horizontal_mean

@@ -32,6 +32,7 @@
  *   ide3d_seg_xent_fwd/_bwd   semantic-mask loss of the projector (extension): cross-entropy of the upsampled logits
  *   ide3d_seg_xent_*_ac       apps/finetune_hybrid_encoder.py:171-174  the same with align_corners=True (BiSeNet's upsampling)
  *   ide3d_lpips_fwd/_bwd      inversion/criteria/lpips/lpips.py:29-35 + utils.py:6-8  LPIPS head over all tapped layers (pivotal tuning)
+ *   ide3d_feat_l1_fwd/_bwd    apps/train_hybrid_encoder.py:143-152  the VGG loss's L1 over all tapped layers (encoder training)
  *   ide3d_seg_stem            Painter/run_UI.py:290-295 + inversion/networks.py:1638-1646  one-hot mask -> stem, conv1 and skip of the
  *                             HybridEncoder's geometry branch, from the class ids through per-class tables (extension)
  *   ide3d_seg_stem_bwd        its gradients w.r.t. the three layers' weights (encoder fine-tuning)
@@ -563,6 +564,42 @@ typedef struct ide3d_lpips_params {
 int64_t ide3d_lpips_scratch_bytes(const ide3d_lpips_params* p);
 int ide3d_lpips_fwd(const ide3d_lpips_params* p, ide3d_stream_t stream);
 int ide3d_lpips_bwd(const ide3d_lpips_params* p, ide3d_stream_t stream);
+
+/* Multi-tap L1 head of the hybrid encoder's VGG loss (apps/train_hybrid_encoder.py:143-152) over every tapped layer of one call:
+ *   total = sum_l weight_l * mean |x_l - y_l|      (the mean over all n * c * h * w elements of layer l)
+ * x, y fp32 [n, c, h, w] with any non-negative element strides (one target per sample).  A layer whose x, y (and grad_x) share one
+ * dense layout -- NCHW or channels_last -- is read as a flat array, with 16-byte accesses when aligned.
+ *   ide3d_feat_l1_fwd: value[l] = the mean of layer l (float), value[num_layers] = total.  Two launches whatever num_layers: one
+ *                      CTA per 4096 elements of a layer sums them into a double partial in a fixed order, one CTA folds the partials
+ *                      of each layer in block order, then the layers in order.  No float atomics: deterministic.  scratch holds
+ *                      the partials (ide3d_feat_l1_scratch_bytes bytes, 8-byte aligned).
+ *   ide3d_feat_l1_bwd: one launch, grad_x_l = grad_value[0] * weight_l / numel_l * sgn(x_l - y_l), 0 where x == y (torch's sgn).
+ *                      grad_value is read on the device.  grad_x uses its own strides.
+ * IDE3D_UNSUPPORTED for num_layers > IDE3D_FEAT_L1_MAX_LAYERS or dtype != IDE3D_F32; IDE3D_INVALID for null pointers, empty sizes
+ * or negative strides. */
+#define IDE3D_FEAT_L1_MAX_LAYERS 8
+typedef struct ide3d_feat_l1_layer {
+    int c, h, w;
+    float weight;
+    const float* x;
+    int64_t x_stride[4];        /* n, c, h, w */
+    const float* y;
+    int64_t y_stride[4];
+    float* grad_x;              /* bwd */
+    int64_t gx_stride[4];
+} ide3d_feat_l1_layer;
+typedef struct ide3d_feat_l1_params {
+    int n, num_layers, dtype;
+    ide3d_feat_l1_layer layers[IDE3D_FEAT_L1_MAX_LAYERS];
+    float* value;               /* fwd: [num_layers + 1] */
+    void* scratch;              /* fwd */
+    int64_t scratch_bytes;
+    const float* grad_value;    /* bwd: [1] */
+} ide3d_feat_l1_params;
+/* bytes of scratch ide3d_feat_l1_fwd needs for this table (negative status for a table it would refuse) */
+int64_t ide3d_feat_l1_scratch_bytes(const ide3d_feat_l1_params* p);
+int ide3d_feat_l1_fwd(const ide3d_feat_l1_params* p, ide3d_stream_t stream);
+int ide3d_feat_l1_bwd(const ide3d_feat_l1_params* p, ide3d_stream_t stream);
 
 /* Opening of the HybridEncoder's geometry branch (inversion/networks.py:1638-1646) from a class-id mask (extension).  The branch's
  * input one_hot(mask) * 2 - 1 takes `classes` + 1 distinct values per pixel (a mask value >= classes is the all-minus-one "no class"
