@@ -12,6 +12,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get('IDE3D_B200_LIB') or os.path.join(_HERE, 'lib', 'libide3d_b200.so')      # (override: A/B runs against a tuning build)
 
+ABI_VERSION = 1                                        # IDE3D_ABI_VERSION
 OK, UNSUPPORTED, INVALID, CUDA_ERROR = 0, -1, -2, -3
 F32, F16, F64 = 0, 1, 2
 JITTER_NONE, JITTER_TENSOR, JITTER_HASH, JITTER_ZVALS = 0, 1, 2, 3
@@ -183,6 +184,66 @@ class SegLabelsParams(C.Structure):
                 ('out_h', C.c_int), ('out_w', C.c_int), ('out', C.c_void_p)]
 
 
+_vp, _i32, _i64, _f32, _P = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.POINTER
+
+# Every function include/ide3d_b200.h declares: name -> (restype, argtypes), in header order.  argtypes None leaves the
+# (void) entry points as ctypes loads them.
+SIGNATURES = {
+    'ide3d_abi_version': (_i32, None),
+    'ide3d_last_error': (C.c_char_p, None),
+    'ide3d_launch_count': (C.c_uint64, None),
+    'ide3d_bias_act': (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _f32, _f32, _f32, _i64, _i64, _i64, _vp]),
+    'ide3d_modconv_epilogue': (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _f32, _f32, _f32, _i64, _i64, _i64, _i64, _i32,
+                                      _vp]),
+    'ide3d_modconv_epilogue_rgb': (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _i32, _f32, _f32,
+                                          _f32, _i64, _i64, _i64, _i64, _vp]),
+    'ide3d_upfirdn2d': (_i32, [_P(UpfirParams), _vp]),
+    'ide3d_upfirdn2d_add': (_i32, [_P(UpfirParams), _vp, _i64, _i64, _i64, _vp, _vp]),
+    'ide3d_upfirdn2d_epilogue': (_i32, [_P(UpfirParams), _P(FirEpilogue), _vp]),
+    'ide3d_filtered_lrelu': (_i32, [_P(FlreluParams), _vp]),
+    'ide3d_filtered_lrelu_act': (_i32, [_P(FlreluActParams), _vp]),
+    'ide3d_raymarch_fwd': (_i32, [_P(RaymarchParams), _vp]),
+    'ide3d_raymarch_bwd': (_i32, [_P(RaymarchParams), _vp, _vp, _vp, _vp, _P(C.c_void_p), _vp]),
+    'ide3d_raymarch_bwd_cam': (_i32, [_P(RaymarchParams), _vp, _vp, _vp, _vp, _P(C.c_void_p), _vp, _vp]),
+    'ide3d_sample_voxel': (_i32, [_P(TriPlane), _P(TriPlane), _P(Decoder), _vp, _i64, _f32, _i32, _vp, _vp]),
+    'ide3d_sigma_grid': (_i32, [_P(TriPlane), _P(TriPlane), _P(Decoder), _i32, _P(C.c_float * 3), _f32, _f32, _f32, _i64, _i64,
+                                _vp, _vp]),
+    'ide3d_planes_to_nhwc': (_i32, [_vp, _i32, _i32, _i32, _i32, _i64, _i64, _i64, _i64, _vp, _vp]),
+    'ide3d_initial_rays': (_i32, [_i32, _i32, _f32, _i32, _i32, _f32, _f32, _vp, _vp, _vp, _vp]),
+    'ide3d_transform_points': (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
+    'ide3d_sample_triplane': (_i32, [_P(TriPlane), _vp, _i64, _vp, _vp]),
+    'ide3d_integrate': (_i32, [_vp, _vp, _vp, _vp, _f32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _f32, _i32, _vp, _vp, _vp, _vp]),
+    'ide3d_sample_pdf': (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _f32, _vp, _vp]),
+    'ide3d_mask2color': (_i32, [_vp, _i32, _i32, _i32, _i32, _i64, _i64, _i64, _i64, _vp, _vp, _i32, _vp]),
+    'ide3d_video_frames': (_i32, [_P(FramesParams), _vp]),
+    'ide3d_image_strips': (_i32, [_P(StripsParams), _vp]),
+    'ide3d_mc_classify': (_i32, [_vp, _i32, _i32, _i32, _f32, _vp, _vp, _vp]),
+    'ide3d_mc_emit': (_i32, [_vp, _i32, _i32, _i32, _f32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    'ide3d_mesh_normals': (_i32, [_vp, _vp, _i64, _vp, _vp, _vp, _vp]),
+    'ide3d_raster_scratch_bytes': (_i64, [_i32, _i32, _i32, _i64, _i64]),
+    'ide3d_raster': (_i32, [_P(RasterParams), _vp]),
+    'ide3d_style_plan': (_i32, [_vp, _i32, _i32, _i32, _P(StyleLayer), _i32, _vp, _vp, _vp]),
+    'ide3d_noise_reg': (_i32, [_P(NoiseTable), _vp, _vp, _vp]),
+    'ide3d_noise_normalize': (_i32, [_P(NoiseTable), _vp]),
+    'ide3d_seg_xent_fwd': (_i32, [_P(SegXentParams), _vp]),
+    'ide3d_seg_xent_bwd': (_i32, [_P(SegXentParams), _vp]),
+    'ide3d_seg_xent_fwd_ac': (_i32, [_P(SegXentParams), _vp]),
+    'ide3d_seg_xent_bwd_ac': (_i32, [_P(SegXentParams), _vp]),
+    'ide3d_lpips_scratch_bytes': (_i64, [_P(LpipsParams)]),
+    'ide3d_lpips_fwd': (_i32, [_P(LpipsParams), _vp]),
+    'ide3d_lpips_bwd': (_i32, [_P(LpipsParams), _vp]),
+    'ide3d_feat_l1_scratch_bytes': (_i64, [_P(FeatL1Params)]),
+    'ide3d_feat_l1_fwd': (_i32, [_P(FeatL1Params), _vp]),
+    'ide3d_feat_l1_bwd': (_i32, [_P(FeatL1Params), _vp]),
+    'ide3d_seg_stem_scratch_bytes': (_i64, [_i32, _i32]),
+    'ide3d_seg_stem': (_i32, [_P(SegStemParams), _vp]),
+    'ide3d_seg_stem_bwd_scratch_bytes': (_i64, [_i32, _i32, _i32, _i32, _i32]),
+    'ide3d_seg_stem_bwd': (_i32, [_P(SegStemBwdParams), _vp]),
+    'ide3d_seg_labels': (_i32, [_P(SegLabelsParams), _vp]),
+    'ide3d_seg_labels_ac': (_i32, [_P(SegLabelsParams), _vp]),
+}
+
+
 _lib = None
 
 
@@ -226,69 +287,10 @@ def get_lib():
         raise RuntimeError(f'ide3d_b200: CUDA library not built ({LIB_PATH} missing); run '
                            f'`python {os.path.join(_HERE, "build.py")}` -- there is no CPU fallback')
     lib = C.CDLL(LIB_PATH, mode=os.RTLD_NOW)       # every symbol resolved at load: a half-built library fails here, loudly
-    lib.ide3d_last_error.restype = C.c_char_p
-    lib.ide3d_launch_count.restype = C.c_uint64
-    vp, i32, i64, f32 = C.c_void_p, C.c_int, C.c_int64, C.c_float
-    lib.ide3d_bias_act.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, f32, f32, f32, i64, i64, i64, vp]
-    lib.ide3d_modconv_epilogue.argtypes = [vp, vp, vp, vp, vp, vp, vp, i32, i32, f32, f32, f32, i64, i64, i64, i64, i32, vp]
-    lib.ide3d_modconv_epilogue_rgb.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i64, i32, i32, f32, f32, f32, i64, i64, i64,
-                                               i64, vp]
-    lib.ide3d_upfirdn2d.argtypes = [C.POINTER(UpfirParams), vp]
-    lib.ide3d_upfirdn2d_add.argtypes = [C.POINTER(UpfirParams), vp, i64, i64, i64, vp, vp]
-    lib.ide3d_upfirdn2d_epilogue.argtypes = [C.POINTER(UpfirParams), C.POINTER(FirEpilogue), vp]
-    lib.ide3d_filtered_lrelu.argtypes = [C.POINTER(FlreluParams), vp]
-    lib.ide3d_filtered_lrelu_act.argtypes = [C.POINTER(FlreluActParams), vp]
-    lib.ide3d_raymarch_fwd.argtypes = [C.POINTER(RaymarchParams), vp]
-    lib.ide3d_raymarch_bwd.argtypes = [C.POINTER(RaymarchParams), vp, vp, vp, vp, C.POINTER(C.c_void_p), vp]
-    lib.ide3d_raymarch_bwd_cam.argtypes = [C.POINTER(RaymarchParams), vp, vp, vp, vp, C.POINTER(C.c_void_p), vp, vp]
-    lib.ide3d_sample_voxel.argtypes = [C.POINTER(TriPlane), C.POINTER(TriPlane), C.POINTER(Decoder), vp, i64, f32, i32, vp, vp]
-    lib.ide3d_sigma_grid.argtypes = [C.POINTER(TriPlane), C.POINTER(TriPlane), C.POINTER(Decoder), i32,
-                                     C.POINTER(C.c_float * 3), f32, f32, f32, i64, i64, vp, vp]
-    lib.ide3d_planes_to_nhwc.argtypes = [vp, i32, i32, i32, i32, i64, i64, i64, i64, vp, vp]
-    lib.ide3d_initial_rays.argtypes = [i32, i32, f32, i32, i32, f32, f32, vp, vp, vp, vp]
-    lib.ide3d_transform_points.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp]
-    lib.ide3d_sample_triplane.argtypes = [C.POINTER(TriPlane), vp, i64, vp, vp]
-    lib.ide3d_mask2color.argtypes = [vp, i32, i32, i32, i32, i64, i64, i64, i64, vp, vp, i32, vp]
-    lib.ide3d_integrate.argtypes = [vp, vp, vp, vp, f32, i32, i32, i32, i32, i32, i32, i32, f32, i32, vp, vp, vp, vp]
-    lib.ide3d_sample_pdf.argtypes = [vp, vp, vp, i32, i32, i32, f32, vp, vp]
-    lib.ide3d_mc_classify.argtypes = [vp, i32, i32, i32, f32, vp, vp, vp]
-    lib.ide3d_mc_emit.argtypes = [vp, i32, i32, i32, f32, vp, vp, vp, vp, vp, vp, vp]
-    lib.ide3d_style_plan.argtypes = [vp, i32, i32, i32, C.POINTER(StyleLayer), i32, vp, vp, vp]
-    lib.ide3d_mesh_normals.argtypes = [vp, vp, i64, vp, vp, vp, vp]
-    lib.ide3d_raster_scratch_bytes.argtypes = [i32, i32, i32, i64, i64]
-    lib.ide3d_raster_scratch_bytes.restype = C.c_int64
-    lib.ide3d_raster.argtypes = [C.POINTER(RasterParams), vp]
-    lib.ide3d_video_frames.argtypes = [C.POINTER(FramesParams), vp]
-    lib.ide3d_image_strips.argtypes = [C.POINTER(StripsParams), vp]
-    lib.ide3d_noise_reg.argtypes = [C.POINTER(NoiseTable), vp, vp, vp]
-    lib.ide3d_noise_normalize.argtypes = [C.POINTER(NoiseTable), vp]
-    lib.ide3d_seg_xent_fwd.argtypes = [C.POINTER(SegXentParams), vp]
-    lib.ide3d_seg_xent_bwd.argtypes = [C.POINTER(SegXentParams), vp]
-    lib.ide3d_seg_xent_fwd_ac.argtypes = [C.POINTER(SegXentParams), vp]
-    lib.ide3d_seg_xent_bwd_ac.argtypes = [C.POINTER(SegXentParams), vp]
-    lib.ide3d_lpips_scratch_bytes.argtypes = [C.POINTER(LpipsParams)]
-    lib.ide3d_lpips_scratch_bytes.restype = C.c_int64
-    lib.ide3d_lpips_fwd.argtypes = [C.POINTER(LpipsParams), vp]
-    lib.ide3d_lpips_bwd.argtypes = [C.POINTER(LpipsParams), vp]
-    lib.ide3d_feat_l1_scratch_bytes.argtypes = [C.POINTER(FeatL1Params)]
-    lib.ide3d_feat_l1_scratch_bytes.restype = C.c_int64
-    lib.ide3d_feat_l1_fwd.argtypes = [C.POINTER(FeatL1Params), vp]
-    lib.ide3d_feat_l1_bwd.argtypes = [C.POINTER(FeatL1Params), vp]
-    lib.ide3d_seg_stem_scratch_bytes.argtypes = [i32, i32]
-    lib.ide3d_seg_stem_scratch_bytes.restype = C.c_int64
-    lib.ide3d_seg_stem.argtypes = [C.POINTER(SegStemParams), vp]
-    lib.ide3d_seg_stem_bwd_scratch_bytes.argtypes = [i32, i32, i32, i32, i32]
-    lib.ide3d_seg_stem_bwd_scratch_bytes.restype = C.c_int64
-    lib.ide3d_seg_stem_bwd.argtypes = [C.POINTER(SegStemBwdParams), vp]
-    lib.ide3d_seg_labels.argtypes = [C.POINTER(SegLabelsParams), vp]
-    lib.ide3d_seg_labels_ac.argtypes = [C.POINTER(SegLabelsParams), vp]
-    for name in ('bias_act', 'upfirdn2d', 'filtered_lrelu', 'filtered_lrelu_act', 'raymarch_fwd', 'raymarch_bwd', 'raymarch_bwd_cam', 'sample_voxel',
-                 'sigma_grid', 'planes_to_nhwc', 'initial_rays', 'transform_points', 'sample_triplane', 'integrate',
-                 'sample_pdf', 'style_plan', 'mc_classify', 'mc_emit', 'mesh_normals', 'raster', 'video_frames', 'image_strips',
-                 'noise_reg', 'noise_normalize', 'seg_xent_fwd', 'seg_xent_bwd', 'seg_xent_fwd_ac', 'seg_xent_bwd_ac', 'lpips_fwd',
-                 'lpips_bwd', 'seg_stem', 'seg_stem_bwd', 'seg_labels', 'seg_labels_ac', 'feat_l1_fwd', 'feat_l1_bwd', 'abi_version'):
-        getattr(lib, 'ide3d_' + name).restype = C.c_int
-    if lib.ide3d_abi_version() != 1:
+    for name, (restype, argtypes) in SIGNATURES.items():
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = restype, argtypes
+    if lib.ide3d_abi_version() != ABI_VERSION:
         raise RuntimeError('ide3d_b200: ABI version mismatch between _lib.py and libide3d_b200.so')
     _lib = _GuardedLib(lib)
     return _lib
@@ -296,16 +298,7 @@ def get_lib():
 
 def exported_symbols():
     """Names declared in include/ide3d_b200.h (used by the CPU test that checks the .so exports them)."""
-    return ['ide3d_abi_version', 'ide3d_last_error', 'ide3d_launch_count', 'ide3d_bias_act', 'ide3d_modconv_epilogue', 'ide3d_modconv_epilogue_rgb',
-            'ide3d_upfirdn2d', 'ide3d_upfirdn2d_add', 'ide3d_upfirdn2d_epilogue',
-            'ide3d_filtered_lrelu', 'ide3d_filtered_lrelu_act', 'ide3d_raymarch_fwd', 'ide3d_raymarch_bwd', 'ide3d_raymarch_bwd_cam', 'ide3d_sample_voxel',
-            'ide3d_sigma_grid', 'ide3d_planes_to_nhwc', 'ide3d_initial_rays', 'ide3d_transform_points',
-            'ide3d_sample_triplane', 'ide3d_integrate', 'ide3d_sample_pdf', 'ide3d_mask2color', 'ide3d_style_plan', 'ide3d_mc_classify', 'ide3d_mc_emit',
-            'ide3d_mesh_normals', 'ide3d_raster_scratch_bytes', 'ide3d_raster', 'ide3d_video_frames', 'ide3d_image_strips',
-            'ide3d_noise_reg', 'ide3d_noise_normalize', 'ide3d_seg_xent_fwd', 'ide3d_seg_xent_bwd',
-            'ide3d_lpips_scratch_bytes', 'ide3d_lpips_fwd', 'ide3d_lpips_bwd', 'ide3d_seg_stem_scratch_bytes', 'ide3d_seg_stem',
-            'ide3d_seg_labels', 'ide3d_seg_xent_fwd_ac', 'ide3d_seg_xent_bwd_ac', 'ide3d_seg_stem_bwd_scratch_bytes', 'ide3d_seg_stem_bwd',
-            'ide3d_seg_labels_ac', 'ide3d_feat_l1_scratch_bytes', 'ide3d_feat_l1_fwd', 'ide3d_feat_l1_bwd']
+    return list(SIGNATURES)
 
 
 def check(rc, allow_unsupported=False):

@@ -1,55 +1,129 @@
-"""CPU: the C-ABI library builds/loads without a GPU and exports every symbol include/ide3d_b200.h declares
-(no compute calls here), and the product refuses CPU tensors instead of falling back."""
+"""CPU: the ctypes mirror in ide3d_b200/_lib.py conforms to include/ide3d_b200.h -- struct pairing and layouts, constants,
+prototypes -- and the library exports every declared function (no compute calls here); the entry points reject malformed
+arguments, and the product refuses CPU tensors instead of falling back."""
 
 import ctypes
 import os
 import re
+import subprocess
 
 import pytest
 import torch
 
 from conftest import ROOT
+from ide3d_b200 import _lib
+
+HEADER = os.path.join(ROOT, 'include', 'ide3d_b200.h')
+
+# header struct -> its ctypes mirror in _lib
+STRUCTS = {
+    'ide3d_upfirdn2d_params': 'UpfirParams', 'ide3d_fir_epilogue': 'FirEpilogue', 'ide3d_filtered_lrelu_params': 'FlreluParams',
+    'ide3d_filtered_lrelu_act_params': 'FlreluActParams', 'ide3d_triplane': 'TriPlane', 'ide3d_mlp_head': 'MlpHead',
+    'ide3d_decoder': 'Decoder', 'ide3d_raymarch_params': 'RaymarchParams', 'ide3d_frames_params': 'FramesParams',
+    'ide3d_strips_params': 'StripsParams', 'ide3d_raster_params': 'RasterParams', 'ide3d_style_layer': 'StyleLayer',
+    'ide3d_noise_table': 'NoiseTable', 'ide3d_seg_xent_params': 'SegXentParams', 'ide3d_lpips_layer': 'LpipsLayer',
+    'ide3d_lpips_params': 'LpipsParams', 'ide3d_feat_l1_layer': 'FeatL1Layer', 'ide3d_feat_l1_params': 'FeatL1Params',
+    'ide3d_seg_stem_params': 'SegStemParams', 'ide3d_seg_stem_bwd_params': 'SegStemBwdParams', 'ide3d_seg_labels_params': 'SegLabelsParams',
+}
+
+# _lib name -> header name of every constant _lib copies from the header
+CONSTANTS = {name: 'IDE3D_' + name for name in (
+    'ABI_VERSION', 'OK', 'UNSUPPORTED', 'INVALID', 'CUDA_ERROR', 'F32', 'F16', 'F64', 'JITTER_NONE', 'JITTER_TENSOR', 'JITTER_HASH',
+    'JITTER_ZVALS', 'CLAMP_SOFTPLUS', 'CLAMP_RELU', 'FRAMES_IMAGE_SEG', 'FRAMES_IMAGE_DEPTH', 'FRAMES_PARTIALS', 'NOISE_MAX_BUFFERS',
+    'LPIPS_MAX_LAYERS', 'FEAT_L1_MAX_LAYERS', 'SEG_STEM_MAX_CLASSES')}
+
+
+def _header():
+    return re.sub(r'/\*.*?\*/', '', open(HEADER).read(), flags=re.S)
 
 
 def header_functions():
-    src = open(os.path.join(ROOT, 'include', 'ide3d_b200.h')).read()
-    src = re.sub(r'/\*.*?\*/', '', src, flags=re.S)
-    return sorted(set(re.findall(r'\b(ide3d_[a-z0-9_]+)\s*\(', src)))
+    """name -> (return type, [parameter declarations]) of every function the header declares."""
+    protos = re.findall(r'^([A-Za-z_][\w \t*]*?)\s*\b(ide3d_\w+)\s*\(([^)]*)\)\s*;', _header(), flags=re.M)
+    return {name: (ret, [] if params.strip() == 'void' else [p.strip() for p in params.split(',')]) for ret, name, params in protos}
+
+
+def c_kind(decl):
+    """'int', 'int64', 'uint64', 'float', 'ptr', or 'ptr:ide3d_x' for a pointer to header struct ide3d_x."""
+    words = [w for w in re.findall(r'\w+|\*|\[', decl) if w != 'const']
+    if '*' in words or '[' in words:
+        return f'ptr:{words[0]}' if words[0] in STRUCTS else 'ptr'
+    return {'int': 'int', 'int64_t': 'int64', 'uint64_t': 'uint64', 'float': 'float', 'ide3d_stream_t': 'ptr'}[words[0]]
+
+
+def ctypes_kind(t):
+    if t in (ctypes.c_void_p, ctypes.c_char_p):
+        return 'ptr'
+    if issubclass(t, ctypes._Pointer):
+        paired = {getattr(_lib, py): c for c, py in STRUCTS.items()}
+        return f'ptr:{paired[t._type_]}' if t._type_ in paired else 'ptr'
+    return {ctypes.c_int: 'int', ctypes.c_int64: 'int64', ctypes.c_uint64: 'uint64', ctypes.c_float: 'float'}[t]
+
+
+@pytest.fixture(scope='module')
+def probe(tmp_path_factory):
+    """Compile and run a C program that prints, from the header, every value the ctypes mirror claims: `key value...` lines."""
+    lines = []
+    for c_name, py_name in STRUCTS.items():
+        lines.append(f'printf("{c_name} %zu %zu\\n", sizeof({c_name}), _Alignof({c_name}));')
+        for field, _ in getattr(_lib, py_name)._fields_:
+            lines.append(f'printf("{c_name}.{field} %zu %zu\\n", offsetof({c_name}, {field}), sizeof((({c_name}*)0)->{field}));')
+    for c_name in list(CONSTANTS.values()) + ['IDE3D_PRECISION_' + k.upper() for k in _lib.PRECISION]:
+        lines.append(f'printf("{c_name} %lld\\n", (long long){c_name});')
+    d = tmp_path_factory.mktemp('abi_probe')
+    (d / 'probe.c').write_text('#include <stddef.h>\n#include <stdio.h>\n#include "ide3d_b200.h"\nint main(void) {\n'
+                               + '\n'.join(lines) + '\nreturn 0;\n}\n')
+    subprocess.run(['gcc', '-std=c11', '-I', os.path.dirname(HEADER), str(d / 'probe.c'), '-o', str(d / 'probe')], check=True)
+    out = subprocess.run([str(d / 'probe')], capture_output=True, text=True, check=True).stdout
+    return {key: [int(v) for v in vals] for key, *vals in (line.split() for line in out.splitlines())}
+
+
+def test_structs_pair_with_header():
+    declared = re.findall(r'\btypedef\s+struct\s+(ide3d_\w+)', _header())
+    assert sorted(declared) == sorted(STRUCTS)
+    mirrors = [name for name, v in vars(_lib).items() if isinstance(v, type) and issubclass(v, ctypes.Structure)]
+    assert sorted(mirrors) == sorted(STRUCTS.values())
+
+
+def test_struct_sizes_match_header(probe):
+    """Every struct's size and alignment, and every field's offset and size, are the C layout."""
+    want = {}
+    for c_name, py_name in STRUCTS.items():
+        cls = getattr(_lib, py_name)
+        want[c_name] = [ctypes.sizeof(cls), ctypes.alignment(cls)]
+        for field, t in cls._fields_:
+            want[f'{c_name}.{field}'] = [getattr(cls, field).offset, ctypes.sizeof(t)]
+    assert {k: probe[k] for k in want} == want
+
+
+def test_constants_match_header(probe):
+    want = {c_name: [getattr(_lib, name)] for name, c_name in CONSTANTS.items()}
+    want.update({'IDE3D_PRECISION_' + k.upper(): [v] for k, v in _lib.PRECISION.items()})
+    assert {k: probe[k] for k in want} == want
+
+
+def test_prototypes_match_header():
+    """The table declares exactly the header's functions, each with the return kind and the parameter kinds of its prototype."""
+    declared = header_functions()
+    assert sorted(declared) == sorted(set(re.findall(r'\b(ide3d_\w+)\s*\(', _header())))      # the parser missed no declaration
+    assert sorted(declared) == sorted(_lib.SIGNATURES)
+    for name, (ret, params) in declared.items():
+        restype, argtypes = _lib.SIGNATURES[name]
+        assert ctypes_kind(restype) == c_kind(ret), name
+        mine = [ctypes_kind(t) for t in argtypes or []]
+        theirs = [c_kind(p) for p in params]
+        assert len(mine) == len(theirs), name
+        # c_void_p stands for any pointer; POINTER(S) must point to the struct of the prototype
+        assert all(m == t or (m == 'ptr' and t.startswith('ptr:')) for m, t in zip(mine, theirs)), (name, mine, theirs)
 
 
 def test_library_exports_every_declared_symbol(lib):
-    names = header_functions()
-    assert len(names) >= 16
-    for n in names:
+    for n in _lib.exported_symbols():
         assert hasattr(lib, n), f'{n} declared in include/ide3d_b200.h but not exported by libide3d_b200.so'
-    from ide3d_b200 import _lib
-    assert sorted(_lib.exported_symbols()) == names
-    assert lib.ide3d_abi_version() == 1
-
-
-def test_struct_sizes_match_header():
-    """ctypes mirrors of the parameter structs must have the C layout (compile a probe with gcc)."""
-    import subprocess, tempfile
-    from ide3d_b200 import _lib
-    probe = r'''
-    #include <stdio.h>
-    #include "ide3d_b200.h"
-    int main(void) { printf("%zu %zu %zu %zu %zu %zu %zu %zu\n", sizeof(ide3d_fir_epilogue), sizeof(ide3d_upfirdn2d_params), sizeof(ide3d_filtered_lrelu_params),
-        sizeof(ide3d_filtered_lrelu_act_params), sizeof(ide3d_triplane), sizeof(ide3d_mlp_head), sizeof(ide3d_decoder),
-        sizeof(ide3d_raymarch_params)); return 0; }'''
-    with tempfile.TemporaryDirectory() as d:
-        c = os.path.join(d, 'p.c')
-        open(c, 'w').write(probe)
-        exe = os.path.join(d, 'p')
-        subprocess.run(['gcc', '-I', os.path.join(ROOT, 'include'), c, '-o', exe], check=True)
-        sizes = [int(v) for v in subprocess.run([exe], capture_output=True, text=True, check=True).stdout.split()]
-    ours = [ctypes.sizeof(t) for t in (_lib.FirEpilogue, _lib.UpfirParams, _lib.FlreluParams, _lib.FlreluActParams, _lib.TriPlane,
-                                       _lib.MlpHead, _lib.Decoder, _lib.RaymarchParams)]
-    assert ours == sizes
+    assert lib.ide3d_abi_version() == _lib.ABI_VERSION
 
 
 def test_invalid_arguments_return_status_not_crash(lib):
-    from ide3d_b200 import _lib
     assert lib.ide3d_raymarch_fwd(None, None) == _lib.INVALID
     assert b'null params' in lib.ide3d_last_error()
     assert lib.ide3d_upfirdn2d(None, None) == _lib.INVALID
@@ -112,7 +186,6 @@ RAYMARCH_BROKEN = {
 def test_raymarch_entry_points_share_validation(lib, case):
     """ide3d_raymarch_fwd and ide3d_raymarch_bwd reject the same malformed parameters with the same status and message,
     before anything reaches the device."""
-    from ide3d_b200 import _lib
     breaker, message = RAYMARCH_BROKEN[case]
     p = _fake_raymarch_params(_lib)
     breaker(p)

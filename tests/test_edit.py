@@ -4,15 +4,12 @@ oracle/edit.py), the table formulation of ide3d_seg_stem, argument validation, a
 
 import ctypes
 import math
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 import torch
 
-from conftest import ROOT, load_golden
+from conftest import load_golden
 
 
 @pytest.fixture(scope='module')
@@ -186,24 +183,6 @@ def test_argument_validation(models, trace):
         edit.reenact(G, E, pivot, label.repeat(2, 1), torch.stack([mask] * 3))
     with pytest.raises(ValueError, match='uint8'):
         E.geometry(mask)
-
-
-def _probe_sizes():
-    probe = r'''
-    #include <stdio.h>
-    #include "ide3d_b200.h"
-    int main(void) { printf("%zu %zu\n", sizeof(ide3d_seg_stem_params), sizeof(ide3d_seg_labels_params)); return 0; }'''
-    with tempfile.TemporaryDirectory() as d:
-        c = os.path.join(d, 'p.c')
-        open(c, 'w').write(probe)
-        exe = os.path.join(d, 'p')
-        subprocess.run(['gcc', '-I', os.path.join(ROOT, 'include'), c, '-o', exe], check=True)
-        return [int(v) for v in subprocess.run([exe], capture_output=True, text=True, check=True).stdout.split()]
-
-
-def test_seg_stem_struct_layout_matches_header():
-    from ide3d_b200 import _lib
-    assert [ctypes.sizeof(_lib.SegStemParams), ctypes.sizeof(_lib.SegLabelsParams)] == _probe_sizes()
 
 
 def test_seg_stem_entry_points_validate_before_the_device(lib):

@@ -7,7 +7,7 @@ import pytest
 import torch
 
 from oracle import renderer as orr
-from test_abi import RAYMARCH_BROKEN, _fake_raymarch_params, header_functions
+from test_abi import RAYMARCH_BROKEN, _fake_raymarch_params
 from test_gpu_renderer import _random_case, three_head_from_dense
 
 S, RES = 12, (6, 5)
@@ -104,12 +104,6 @@ def test_hierarchical_gradient_is_the_fine_pass_with_detached_depths():
     for mine, ref, what in ((t.grad, gt, 'tex'), (s.grad, gs, 'seg'), (c.grad, gc, 'cam')):
         assert (mine - ref).abs().max() <= tol(ref), what
     check_head_grads(heads, gp, tol)
-
-
-def test_camera_backward_symbol_is_exported(lib):
-    from ide3d_b200 import _lib
-    assert 'ide3d_raymarch_bwd_cam' in header_functions() and 'ide3d_raymarch_bwd_cam' in _lib.exported_symbols()
-    assert hasattr(lib, 'ide3d_raymarch_bwd_cam')
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason='passes fake device pointers: run only where no GPU can be reached')

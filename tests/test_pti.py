@@ -3,15 +3,12 @@ the stand-ins of oracle/projector.py and oracle/pti.py), lpips_head_torch agains
 validation, the free-view cameras, and the ABI of the LPIPS kernels."""
 
 import ctypes
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 import torch
 
-from conftest import ROOT, load_golden
+from conftest import load_golden
 
 RUNS = {'w': 'w', 'w_plus': 'w_plus', 'join_view': 'join_view', 'early_stop': 'w'}
 
@@ -208,24 +205,6 @@ def test_invalidate_caches_drops_every_cache():
     assert all('_const_cache' not in m.__dict__ for m in layers)
     assert G.synthesis.renderer._packed is None and G.synthesis.renderer._packed_key is None
     assert G.synthesis not in triplane._STYLE_PLANS
-
-
-def _probe_sizes():
-    probe = r'''
-    #include <stdio.h>
-    #include "ide3d_b200.h"
-    int main(void) { printf("%zu %zu\n", sizeof(ide3d_lpips_layer), sizeof(ide3d_lpips_params)); return 0; }'''
-    with tempfile.TemporaryDirectory() as d:
-        c = os.path.join(d, 'p.c')
-        open(c, 'w').write(probe)
-        exe = os.path.join(d, 'p')
-        subprocess.run(['gcc', '-I', os.path.join(ROOT, 'include'), c, '-o', exe], check=True)
-        return [int(v) for v in subprocess.run([exe], capture_output=True, text=True, check=True).stdout.split()]
-
-
-def test_lpips_struct_layout_matches_header():
-    from ide3d_b200 import _lib
-    assert [ctypes.sizeof(_lib.LpipsLayer), ctypes.sizeof(_lib.LpipsParams)] == _probe_sizes()
 
 
 def test_lpips_entry_points_validate_before_the_device(lib):

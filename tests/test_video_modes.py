@@ -4,9 +4,7 @@ recording, and the C-ABI argument checks of ide3d_video_frames."""
 
 import ctypes
 import os
-import subprocess
 import sys
-import tempfile
 
 import numpy as np
 import pytest
@@ -193,20 +191,3 @@ def test_video_frames_abi_validates_before_touching_the_device(lib):
     assert call(**dict(seg, n=0)) == _lib.OK and call(**dict(depth, n=0)) == _lib.OK                # empty batch: nothing to do
     assert call(**seg) == _lib.INVALID and b'null' in lib.ide3d_last_error()                         # null tensors
     assert call(**depth) == _lib.INVALID and b'null' in lib.ide3d_last_error()
-
-
-def test_frames_params_layout_matches_header():
-    from ide3d_b200 import _lib
-    probe = r'''
-    #include <stdio.h>
-    #include <stddef.h>
-    #include "ide3d_b200.h"
-    int main(void) { printf("%zu %zu %zu %zu %d\n", sizeof(ide3d_frames_params), offsetof(ide3d_frames_params, seg_stride_n),
-        offsetof(ide3d_frames_params, scratch), offsetof(ide3d_frames_params, mode), IDE3D_FRAMES_PARTIALS); return 0; }'''
-    with tempfile.TemporaryDirectory() as d:
-        src, exe = os.path.join(d, 'p.c'), os.path.join(d, 'p')
-        open(src, 'w').write(probe)
-        subprocess.run(['gcc', '-I', os.path.join(ROOT, 'include'), src, '-o', exe], check=True)
-        got = [int(v) for v in subprocess.run([exe], capture_output=True, text=True, check=True).stdout.split()]
-    P = _lib.FramesParams
-    assert got == [ctypes.sizeof(P), P.seg_stride_n.offset, P.scratch.offset, P.mode.offset, _lib.FRAMES_PARTIALS]
