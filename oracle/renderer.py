@@ -2,6 +2,8 @@
 
 torch-CPU fp32, written from the reference's Python functions (cited per function).  Used only as
 the checker for the CUDA kernels and as the CPU baseline leg of bench.py -- never shipped.
+The render chain follows the dtype and device of its inputs (the planes for render_frames), so the
+same functions give a float64 reference on the GPU; fp32 CPU inputs take exactly the fp32 CPU ops.
 
 Reference files followed (relative to the reference tree):
   training/volumetric_rendering.py   rays :77-97, jitter :99-105, world transform :108-136,
@@ -25,21 +27,21 @@ N_OUT = 52       # 32 colour features + 19 semantic logits + 1 sigma (extract_sh
 
 # ----------------------------------------------------------------------------- rays (a1)
 
-def initial_rays(n, num_steps, fov, resolution, ray_start, ray_end):
+def initial_rays(n, num_steps, fov, resolution, ray_start, ray_end, dtype=None, device=None):
     """get_initial_rays_trig, volumetric_rendering.py:77-97.
 
     Pixel i = py*W + px; x sweeps -1..1 along px, y sweeps +1..-1 along py (the reference builds a
     meshgrid with default 'ij' indexing and then transposes, :83-86).  Returns
-    points [n,HW,S,3], z_vals [n,HW,S,1], rays_d_cam [n,HW,3]."""
+    points [n,HW,S,3], z_vals [n,HW,S,1], rays_d_cam [n,HW,3] of the given dtype and device (None: torch's defaults)."""
     W, H = resolution
-    xs = torch.linspace(-1, 1, W)
-    ys = torch.linspace(1, -1, H)
+    xs = torch.linspace(-1, 1, W, dtype=dtype, device=device)
+    ys = torch.linspace(1, -1, H, dtype=dtype, device=device)
     x = xs.reshape(1, W).expand(H, W).reshape(-1)
     y = ys.reshape(H, 1).expand(H, W).reshape(-1)
     z = -torch.ones_like(x) / np.tan((2 * math.pi * fov / 360) / 2)
     d = torch.stack([x, y, z], -1)
     d = d / torch.norm(d, dim=-1, keepdim=True)
-    zv = torch.linspace(ray_start, ray_end, num_steps).reshape(1, num_steps, 1).repeat(W * H, 1, 1)
+    zv = torch.linspace(ray_start, ray_end, num_steps, dtype=dtype, device=device).reshape(1, num_steps, 1).repeat(W * H, 1, 1)
     pts = d.unsqueeze(1).repeat(1, num_steps, 1) * zv
     return (pts.unsqueeze(0).repeat(n, 1, 1, 1).contiguous(),
             zv.unsqueeze(0).repeat(n, 1, 1, 1).contiguous(),
@@ -84,11 +86,11 @@ def to_world(points, dirs, cam2world):
     """transform_sampled_points, volumetric_rendering.py:122-134 (camera given => sampled pose is
     discarded, :119-120).  Returns points_world [n,HW,S,3], dirs_world [n,HW,3], origins [n,HW,3]."""
     n, R, S, _ = points.shape
-    hom = torch.ones((n, R, S, 4))
+    hom = torch.ones((n, R, S, 4), dtype=cam2world.dtype, device=cam2world.device)
     hom[..., :3] = points
     pw = torch.bmm(cam2world, hom.reshape(n, -1, 4).permute(0, 2, 1)).permute(0, 2, 1).reshape(n, R, S, 4)
     dw = torch.bmm(cam2world[..., :3, :3], dirs.reshape(n, -1, 3).permute(0, 2, 1)).permute(0, 2, 1).reshape(n, R, 3)
-    ho = torch.zeros((n, 4, R))
+    ho = torch.zeros((n, 4, R), dtype=cam2world.dtype, device=cam2world.device)
     ho[:, 3, :] = 1
     ow = torch.bmm(cam2world, ho).permute(0, 2, 1).reshape(n, R, 4)[..., :3]
     return pw[..., :3], dw, ow
@@ -110,7 +112,7 @@ def bilinear_zeros(plane, u, v):
     x0 = x0.long()
     y0 = y0.long()
     flat = plane.reshape(N, C, H * W)
-    out = torch.zeros((N, u.shape[1], C), dtype=plane.dtype)
+    out = torch.zeros((N, u.shape[1], C), dtype=plane.dtype, device=plane.device)
     taps = ((0, 0, (1 - fx) * (1 - fy)), (0, 1, fx * (1 - fy)), (1, 0, (1 - fx) * fy), (1, 1, fx * fy))
     for dy, dx, w in taps:
         xx = x0 + dx
@@ -156,11 +158,16 @@ class Decoder:
         o = W2 @ h + b2                W2 [52,HID]     o = (32 colour, 19 semantic, 1 sigma)
 
     The generator's three heads (texture->colour, shape->semantic, shape->sigma) are block-sparse
-    instances of this dense form (see ide3d_b200.training.triplane.TriPlaneDecoder.packed())."""
+    instances of this dense form (see ide3d_b200.training.triplane.TriPlaneDecoder.packed()).
+    Floating-point torch tensors keep their dtype and device; anything else becomes fp32 on the CPU."""
 
     def __init__(self, w1, b1, w2, b2):
-        self.w1, self.b1, self.w2, self.b2 = [torch.as_tensor(t, dtype=torch.float32) for t in (w1, b1, w2, b2)]
+        dtype = w1.dtype if torch.is_tensor(w1) and w1.is_floating_point() else torch.float32
+        self.w1, self.b1, self.w2, self.b2 = [torch.as_tensor(t, dtype=dtype) for t in (w1, b1, w2, b2)]
         assert self.w1.shape[1] == 2 * N_FEAT and self.w2.shape == (N_OUT, self.w1.shape[0])
+
+    def to(self, dtype=None, device=None):
+        return Decoder(*[t.to(dtype=dtype, device=device) for t in (self.w1, self.b1, self.w2, self.b2)])
 
     @staticmethod
     def random(hidden=64, seed=0, three_head=True):
@@ -232,7 +239,7 @@ def sample_pdf(bins, weights, n_importance, det=False, eps=1e-5, u=None):
     cdf = torch.cumsum(pdf, -1)
     cdf = torch.cat([torch.zeros_like(cdf[:, :1]), cdf], -1)
     if det:
-        u = torch.linspace(0, 1, n_importance).expand(n_rays, n_importance)
+        u = torch.linspace(0, 1, n_importance, dtype=weights.dtype, device=weights.device).expand(n_rays, n_importance)
     assert u is not None
     u = u.contiguous()
     inds = torch.searchsorted(cdf, u)
@@ -259,20 +266,29 @@ def sample_voxel(planes_tex, planes_seg, decoder, points, box_scale=2.0):
 def render_frames(planes_tex, planes_seg, decoder, cam2world, fov=18.0, num_steps=48, ray_start=2.25,
                   ray_end=3.3, resolution=(64, 64), box_scale=2.0, jitter_u=None, jitter_seed=None,
                   clamp_mode='softplus', last_back=False, white_back=False, max_depth=None,
-                  fill_mode=None, noise=None, noise_std=0.0, return_stages=False):
+                  fill_mode=None, noise=None, noise_std=0.0, return_stages=False, gather=sample_triplane):
     """a1 -> a2 -> a3 -> a5 x2 -> a6 -> a7, the chain the absent generator class runs per frame.
-    jitter_u: explicit [N,HW,S,1] uniforms; jitter_seed: use hash_uniform(seed); neither: no jitter."""
+    jitter_u: explicit [N,HW,S,1] uniforms; jitter_seed: use hash_uniform(seed); neither: no jitter.
+    Rays and camera take the planes' dtype and device; jitter_u and noise are moved to that device.
+    gather: sample_triplane (the explicit restatement) or sample_triplane_torch (F.grid_sample, whose
+    autograd saves the grid instead of four [N,C,P] gathers per plane: the memory-light form for a
+    float64 reference at full size)."""
     N = planes_tex.shape[0]
     W, H = resolution
-    pts, zv, d = initial_rays(N, num_steps, fov, resolution, ray_start, ray_end)
+    dtype, dev = planes_tex.dtype, planes_tex.device
+    pts, zv, d = initial_rays(N, num_steps, fov, resolution, ray_start, ray_end, dtype=dtype, device=dev)
     if jitter_u is None and jitter_seed is not None:
         idx = np.arange(N * W * H * num_steps, dtype=np.uint64)
         jitter_u = torch.from_numpy(hash_uniform(idx, jitter_seed)).reshape(N, W * H, num_steps, 1)
+    if jitter_u is not None:
+        jitter_u = jitter_u.to(device=dev)
+    if noise is not None:
+        noise = noise.to(device=dev)
     pts, zv = perturb(pts, zv, d, jitter_u)
-    pw, dw, ow = to_world(pts, d, cam2world.float())
+    pw, dw, ow = to_world(pts, d, cam2world.to(device=dev, dtype=dtype))
     coords = pw.reshape(N, -1, 3) * box_scale
-    f_tex = sample_triplane(coords, planes_tex)
-    f_seg = sample_triplane(coords, planes_seg)
+    f_tex = gather(coords, planes_tex)
+    f_seg = gather(coords, planes_seg)
     out = decoder(f_tex, f_seg).reshape(N, W * H, num_steps, N_OUT)
     rgb, depth, weights = composite(out, d, zv, noise=noise, noise_std=noise_std, last_back=last_back,
                                     white_back=white_back, max_depth=max_depth, clamp_mode=clamp_mode,
@@ -302,8 +318,9 @@ def render_frames_hierarchical(planes_tex, planes_seg, decoder, cam2world, fov=1
                        resolution=resolution, box_scale=box_scale, jitter_u=jitter_u, jitter_seed=jitter_seed,
                        clamp_mode=clamp_mode, return_stages=True)
     zv, w = st['z_vals'], st['weights']                                   # [N,HW,S,1]
-    _, _, d = initial_rays(N, S, fov, resolution, ray_start, ray_end)
-    _, dw, ow = to_world(torch.zeros(N, W * H, 1, 3), d, cam2world.float())
+    dtype, dev = planes_tex.dtype, planes_tex.device
+    _, _, d = initial_rays(N, S, fov, resolution, ray_start, ray_end, dtype=dtype, device=dev)
+    _, dw, ow = to_world(torch.zeros(N, W * H, 1, 3, dtype=dtype, device=dev), d, cam2world.to(device=dev, dtype=dtype))
     z = zv.reshape(N * W * H, S)
     z_mid = 0.5 * (z[:, :-1] + z[:, 1:])
     fine = sample_pdf(z_mid, w.reshape(N * W * H, S)[:, 1:-1] + 1e-5, n_imp, det=det, u=importance_u).reshape(N, W * H, n_imp, 1)

@@ -67,11 +67,13 @@ def _planes(n, plane, g, smooth):
     """White noise is the adversarial input for an fp32 gather: a texel-to-texel slope of O(1) turns the ~3e-7 rounding
     of the world coordinates (cancellation in cam2world: |R p| ~ 3 against t = 2.7) into plane_res * 3e-7 * slope of
     feature error on EITHER implementation.  Generator planes are smooth; `smooth` draws band-limited noise
-    (8x8 control points, bicubic) so that the tight tolerance measures the kernel and not that conditioning."""
+    (8x8 control points, bicubic) so that the tight tolerance measures the kernel and not that conditioning.
+    plane: side of square planes, or (H, W)."""
+    size = (plane, plane) if isinstance(plane, int) else tuple(plane)
     if not smooth:
-        return torch.randn(n, 96, plane, plane, generator=g)
+        return torch.randn(n, 96, *size, generator=g)
     lo = torch.randn(n, 96, 8, 8, generator=g)
-    return torch.nn.functional.interpolate(lo, size=(plane, plane), mode='bicubic', align_corners=True).contiguous()
+    return torch.nn.functional.interpolate(lo, size=size, mode='bicubic', align_corners=True).contiguous()
 
 
 def _random_case(n, plane, seed, hidden=64, three_head=True, smooth=True):

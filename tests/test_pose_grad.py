@@ -20,14 +20,16 @@ def cfg_for(S_, **opts):
                 white_back=opts.get('white_back', False), max_depth=opts.get('max_depth', 0.0), fill_weight=opts.get('fill_mode') == 'weight')
 
 
-def oracle_explicit(tex, seg, dec, cam, z, box_scale=2.0, **opts):
-    """initial_rays (directions) -> points d * z at the given depths [n,R,S] -> to_world -> sample_triplane -> decoder -> composite."""
-    n, _, S_ = z.shape
-    _, _, d = orr.initial_rays(n, S_, 18.0, RES, 2.25, 3.3)
-    zz = z.reshape(n, R, S_, 1)
-    pw, _, _ = orr.to_world(d.unsqueeze(2) * zz, d, cam)
+def oracle_explicit(tex, seg, dec, cam, z, box_scale=2.0, res=RES, gather=orr.sample_triplane, **opts):
+    """initial_rays (directions) -> points d * z at the given depths [n,R,S] -> to_world -> gather -> decoder -> composite.
+    Rays, depths and camera take the planes' dtype and device (a float64 reference on the GPU: gather=orr.sample_triplane_torch)."""
+    n, R_, S_ = z.shape
+    assert R_ == res[0] * res[1]
+    _, _, d = orr.initial_rays(n, S_, 18.0, res, 2.25, 3.3, dtype=tex.dtype, device=tex.device)
+    zz = z.to(device=tex.device, dtype=tex.dtype).reshape(n, R_, S_, 1)
+    pw, _, _ = orr.to_world(d.unsqueeze(2) * zz, d, cam.to(device=tex.device, dtype=tex.dtype))
     coords = pw.reshape(n, -1, 3) * box_scale
-    out = dec(orr.sample_triplane(coords, tex), orr.sample_triplane(coords, seg)).reshape(n, R, S_, orr.N_OUT)
+    out = dec(gather(coords, tex), gather(coords, seg)).reshape(n, R_, S_, orr.N_OUT)
     return orr.composite(out, d, zz, **dict(dict(clamp_mode='softplus'), **opts))
 
 
