@@ -22,6 +22,11 @@ PRECISION = {'auto': 0, 'fp32': 1, 'tc': 2}
 _DTYPES = {torch.float32: F32, torch.float16: F16, torch.float64: F64}
 
 
+def dtype2(a, b):
+    """IDE3D_DTYPE2(a, b): the mixed-format code of the epilogues and the skip add (torch dtypes in, int out)."""
+    return _DTYPES[a] | ((_DTYPES[b] + 1) << 4)
+
+
 class UpfirParams(C.Structure):
     _fields_ = [('x', C.c_void_p), ('f', C.c_void_p), ('y', C.c_void_p), ('dtype', C.c_int),
                 ('up_x', C.c_int), ('up_y', C.c_int), ('down_x', C.c_int), ('down_y', C.c_int),

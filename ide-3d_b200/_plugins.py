@@ -60,18 +60,22 @@ def bias_act(x, b, xref, yref, dy, grad, dim, act, alpha, gain, clamp):
     return y
 
 
-def modconv_epilogue(x, scale, noise, b, act, alpha, gain, clamp, next_scale=None, only_next=False):
+def modconv_epilogue(x, scale, noise, b, act, alpha, gain, clamp, next_scale=None, only_next=False, out_dtype=None):
     """bias_act(x * scale[:, :, None, None] + noise, b) in one pass (extension, forward only).  x [N,C,H,W] dense NCHW or
     channels_last; scale [N,C] | None; noise [H,W] / [1,1,H,W] / [N,1,H,W] | None; b [C] | None.  With next_scale [N,C] a
     second tensor y * next_scale[:, :, None, None] is written in the same pass -> (y, y2), or y2 alone if only_next.
-    Returns None when the kernel does not take the shape (caller composes the reference ops instead)."""
+    out_dtype torch.float16 (channels_last float32 x, linear / lrelu): y and y2 are written in fp16, each rounded once from the
+    float32 result.  Returns None when the kernel does not take the shape (caller composes the reference ops instead)."""
     L.require_cuda(x)
     _req(x.ndim == 4, 'x must be rank 4')
     n, c, h, w = x.shape
     cl = (not x.is_contiguous()) and x.is_contiguous(memory_format=torch.channels_last)
     _req(x.is_contiguous() or cl, 'x must be non-overlapping and dense')
+    out_dtype = x.dtype if out_dtype is None else out_dtype
+    mixed = out_dtype != x.dtype
+    _req(not mixed or (x.dtype == torch.float32 and out_dtype == torch.float16), 'out_dtype must be the dtype of x, or float16 for float32 x')
     vec = 16 // x.element_size()
-    if x.numel() == 0 or (cl and c % vec != 0) or (not cl and (h * w) % vec != 0):
+    if x.numel() == 0 or (cl and c % vec != 0) or (not cl and (h * w) % vec != 0) or (mixed and (not cl or act not in (1, 3))):
         return None
     if _has(scale):
         _req(scale.numel() == n * c, 'scale must have N*C elements')
@@ -88,13 +92,14 @@ def modconv_epilogue(x, scale, noise, b, act, alpha, gain, clamp, next_scale=Non
     if _has(next_scale):
         _req(next_scale.numel() == n * c, 'next_scale must have N*C elements')
         next_scale = next_scale.to(dtype=x.dtype).reshape(n, c).contiguous()
-        y2 = torch.empty_like(x)
+        y2 = torch.empty_like(x, dtype=out_dtype)
     if not (only_next and y2 is not None):
-        y = torch.empty_like(x)
+        y = torch.empty_like(x, dtype=out_dtype)
     rc = L.get_lib().ide3d_modconv_epilogue(L.ptr(x), L.ptr(scale) if _has(scale) else None, L.ptr(noise) if _has(noise) else None,
                                             L.ptr(b) if _has(b) else None, L.ptr(y) if y is not None else None,
                                             L.ptr(next_scale) if y2 is not None else None, L.ptr(y2) if y2 is not None else None,
-                                            L.dtype_code(x), int(act), float(alpha), float(gain), float(clamp), n, c, h * w,
+                                            L.dtype2(x.dtype, out_dtype) if mixed else L.dtype_code(x), int(act), float(alpha),
+                                            float(gain), float(clamp), n, c, h * w,
                                             noise_batch, int(cl), L.stream_ptr(x.device))
     if L.check(rc, allow_unsupported=True) == L.UNSUPPORTED:
         return None
@@ -103,34 +108,36 @@ def modconv_epilogue(x, scale, noise, b, act, alpha, gain, clamp, next_scale=Non
     return y2 if y is None else (y, y2)
 
 
-def modconv_epilogue_rgb(x, scale, noise, b, act, alpha, gain, clamp, emit_y=True, y_scale=None, next_scale=None, rgb=None):
-    """`modconv_epilogue` for channels_last float32 x with the consumers of its output folded in (extension, forward only):
+def modconv_epilogue_rgb(x, scale, noise, b, act, alpha, gain, clamp, emit_y=True, y_scale=None, next_scale=None, rgb=None, fp32_tail=False):
+    """`modconv_epilogue` for channels_last x with the consumers of its output folded in (extension, forward only):
     y = t (* y_scale[:, :, None, None]) if emit_y; y2 = t * next_scale[:, :, None, None] if next_scale is given; with
     rgb = (weight [O,C,1,1], styles [N,C], bias [O] | None), O <= 4, the ToRGB output conv1x1(t * styles, weight) + bias as a dense
-    NCHW [N,O,H,W] tensor.  Returns the list of the requested outputs in the order (y, y2, rgb), or None when the kernel does
-    not take the shape (caller composes the reference ops instead)."""
+    NCHW [N,O,H,W] float32 tensor.  x float32, or with fp32_tail float16 (the output of an fp16 convolution; y and y2 are then
+    fp16, each rounded once from the float32 result).  Every other operand is used in float32.  Returns the list of the requested outputs in the
+    order (y, y2, rgb), or None when the kernel does not take the shape (caller composes the reference ops instead)."""
     L.require_cuda(x)
     _req(x.ndim == 4, 'x must be rank 4')
     n, c, h, w = x.shape
     cl = (not x.is_contiguous()) and x.is_contiguous(memory_format=torch.channels_last)
-    if not cl or x.dtype != torch.float32 or c % 4 != 0 or c > 512 or x.numel() == 0:
+    if not cl or x.dtype != (torch.float16 if fp32_tail else torch.float32) or c % 4 != 0 or c > 512 or x.numel() == 0:
         return None
+    f32 = torch.float32
 
     def per_sample(t, name):
         if not _has(t):
             return None
         _req(t.numel() == n * c, f'{name} must have N*C elements')
-        return t.to(dtype=x.dtype).reshape(n, c).contiguous()
+        return t.to(dtype=f32).reshape(n, c).contiguous()
 
     scale, y_scale, next_scale = per_sample(scale, 'scale'), per_sample(y_scale, 'y_scale'), per_sample(next_scale, 'next_scale')
     noise_batch = 1
     if _has(noise):
         _req(noise.numel() in (h * w, n * h * w), 'noise must be [H,W] or [N,1,H,W]')
         noise_batch = noise.numel() // (h * w)
-        noise = noise.to(dtype=x.dtype).contiguous()
+        noise = noise.to(dtype=f32).contiguous()
     if _has(b):
         _req(b.ndim == 1 and b.shape[0] == c, 'b has wrong number of elements')
-        b = b.to(dtype=x.dtype).contiguous()
+        b = b.to(dtype=f32).contiguous()
     _req(y_scale is None or emit_y, 'y_scale needs emit_y')
     wrgb = srgb = brgb = out_rgb = None
     o = 0
@@ -140,18 +147,19 @@ def modconv_epilogue_rgb(x, scale, noise, b, act, alpha, gain, clamp, emit_y=Tru
         if o > 4:
             return None
         _req(wrgb.numel() == o * c, 'rgb weight must be [O, C, 1, 1]')
-        wrgb = wrgb.to(dtype=x.dtype).reshape(o, c).contiguous()
+        wrgb = wrgb.to(dtype=f32).reshape(o, c).contiguous()
         srgb = per_sample(srgb, 'rgb styles')
         if brgb is not None:
             _req(brgb.numel() == o, 'rgb bias must have O elements')
-            brgb = brgb.to(dtype=x.dtype).contiguous()
-        out_rgb = torch.empty([n, o, h, w], dtype=x.dtype, device=x.device)
+            brgb = brgb.to(dtype=f32).contiguous()
+        out_rgb = torch.empty([n, o, h, w], dtype=f32, device=x.device)
     y = torch.empty_like(x) if emit_y else None
     y2 = torch.empty_like(x) if next_scale is not None else None
     _req(y is not None or y2 is not None or out_rgb is not None, 'no output requested')
     opt = lambda t: L.ptr(t) if t is not None else None
     rc = L.get_lib().ide3d_modconv_epilogue_rgb(L.ptr(x), opt(scale), opt(noise), opt(b), opt(y_scale), opt(y), opt(next_scale), opt(y2),
-                                                opt(wrgb), opt(srgb), opt(brgb), opt(out_rgb), o, L.dtype_code(x), int(act), float(alpha),
+                                                opt(wrgb), opt(srgb), opt(brgb), opt(out_rgb), o,
+                                                L.F32 if x.dtype == f32 else L.dtype2(x.dtype, x.dtype), int(act), float(alpha),
                                                 float(gain), float(clamp), n, c, h * w, noise_batch, L.stream_ptr(x.device))
     if L.check(rc, allow_unsupported=True) == L.UNSUPPORTED:
         return None
@@ -162,8 +170,10 @@ def modconv_epilogue_rgb(x, scale, noise, b, act, alpha, gain, clamp, emit_y=Tru
 def upfirdn2d(x, f, upx, upy, downx, downy, padx0, padx1, pady0, pady1, flip, gain, add=None, bias=None, epilogue=None):
     """Extensions (return None if the kernel cannot fuse them, so the caller composes the reference ops):
     add / bias: y = upfirdn2d(x) + add + bias[c] in one pass;
-    epilogue = dict(scale, noise, b, act (1|3), alpha, gain, clamp, next_scale, only_next): the modulated-convolution tail applied
-    to the filter output, -> y | (y, y2) | y2 exactly like `modconv_epilogue`."""
+    epilogue = dict(scale, noise, b, act (1|3), alpha, gain, clamp, next_scale, only_next, fp32_tail): the modulated-convolution tail
+    applied to the filter output, -> y | (y, y2) | y2 exactly like `modconv_epilogue`; with fp32_tail and fp16 x the tail operands
+    stay float32 (y / y2 fp16, rounded once), else they take the dtype of x.
+    add of another dtype than x: float16 add onto float32 x."""
     L.require_cuda(x, f)
     _req(f.device == x.device, 'f must reside on the same device as x')
     _req(f.dtype == torch.float32, 'f must be float32')
@@ -188,18 +198,23 @@ def upfirdn2d(x, f, upx, upy, downx, downy, padx0, padx1, pady0, pady1, flip, ga
         e = epilogue
         if not (y.is_contiguous(memory_format=torch.channels_last) and not y.is_contiguous()) or e['act'] not in (1, 3) or x.dtype == torch.float64:
             return None
+        tail = torch.float32 if e.get('fp32_tail') else x.dtype
+        if tail != x.dtype:
+            _req(x.dtype == torch.float16, 'fp32_tail needs float16 x')
+            p.dtype = L.dtype2(x.dtype, x.dtype)
+
         def prep(t, numel):
             if t is None:
                 return None
             _req(t.numel() == numel, 'epilogue operand has the wrong number of elements')
-            return t.to(dtype=x.dtype).contiguous()
+            return t.to(dtype=tail).contiguous()
         scale, b, scale2 = prep(e.get('scale'), n * c), prep(e.get('b'), c), prep(e.get('next_scale'), n * c)
         noise = e.get('noise')
         noise_batch = 1
         if noise is not None:
             _req(noise.numel() in (out_h * out_w, n * out_h * out_w), 'noise must be [H,W] or [N,1,H,W]')
             noise_batch = noise.numel() // (out_h * out_w)
-            noise = noise.to(dtype=x.dtype).contiguous()
+            noise = noise.to(dtype=tail).contiguous()
         y2 = torch.empty_like(y) if scale2 is not None else None
         want_y = not (e.get('only_next') and y2 is not None)
         if not want_y:
@@ -215,8 +230,11 @@ def upfirdn2d(x, f, upx, upy, downx, downy, padx0, padx1, pady0, pady1, flip, ga
             return y
         return (y, y2) if want_y else y2
     if add is not None:
-        if tuple(add.shape) != (n, c, out_h, out_w) or add.dtype != x.dtype or add.stride(1) != 1 or not y.is_contiguous(memory_format=torch.channels_last) or y.is_contiguous():
+        mixed = add.dtype == torch.float16 and x.dtype == torch.float32
+        if tuple(add.shape) != (n, c, out_h, out_w) or (add.dtype != x.dtype and not mixed) or add.stride(1) != 1 or not y.is_contiguous(memory_format=torch.channels_last) or y.is_contiguous():
             return None
+        if mixed:
+            p.dtype = L.dtype2(x.dtype, add.dtype)
         if bias is not None:
             bias = bias.to(dtype=x.dtype).contiguous()
         a = add.stride()

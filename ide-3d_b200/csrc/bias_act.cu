@@ -3,6 +3,8 @@
 // (bias_act.h:12-31).  Pure HBM stream: 2 * size_x * sizeof(T) algorithmic bytes (+ aux tensors for
 // the gradient forms).  128-bit loads/stores, 4 vectors in flight per thread, 64-bit indexing, grid
 // sized to the SM count (grid-stride loop).
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace ide3d {
@@ -114,11 +116,20 @@ __device__ __forceinline__ void load_vec(const __half* p, long long v, float (&o
         o[2 * i] = f.x; o[2 * i + 1] = f.y;
     }
 }
+__device__ __forceinline__ void load_vec(const __half* p, long long v, float (&o)[4]) {
+    const uint2 t = __ldcs(reinterpret_cast<const uint2*>(p) + v);
+    const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&t.x)), b = __half22float2(*reinterpret_cast<const __half2*>(&t.y));
+    o[0] = a.x; o[1] = a.y; o[2] = b.x; o[3] = b.y;
+}
 __device__ __forceinline__ void store_vec(float* p, long long v, const float (&o)[4]) {
     __stcs(reinterpret_cast<float4*>(p) + v, make_float4(o[0], o[1], o[2], o[3]));
 }
 __device__ __forceinline__ void store_vec(double* p, long long v, const double (&o)[2]) {
     __stcs(reinterpret_cast<double2*>(p) + v, make_double2(o[0], o[1]));
+}
+__device__ __forceinline__ void store_vec(__half* p, long long v, const float (&o)[4]) {    // 4 channels, rounded once each
+    const __half2 a = __floats2half2_rn(o[0], o[1]), b = __floats2half2_rn(o[2], o[3]);
+    __stcs(reinterpret_cast<uint2*>(p) + v, make_uint2(*reinterpret_cast<const unsigned*>(&a), *reinterpret_cast<const unsigned*>(&b)));
 }
 __device__ __forceinline__ void store_vec(__half* p, long long v, const float (&o)[8]) {
     unsigned w[4];
@@ -385,7 +396,8 @@ __global__ void __launch_bounds__(256) modconv_epilogue_planar_kernel(const EpiA
 // Work items are (sample, chunk of 256*UNROLL vectors): the sample index is block-uniform and the position inside the
 // sample fits 32 bits, so the per-vector index math is one shift/mask (power-of-two channel counts) or one 32-bit division
 // -- the first version spent 3/4 of its issue slots on 64-bit div/mod.
-template <typename T, int A, int UNROLL>
+// TO: type of y / y2 -- T, or __half for float32 x (the fp16 operand of the next convolution, rounded once from the fp32 value).
+template <typename T, typename TO, int A, int UNROLL>
 __global__ void __launch_bounds__(256) modconv_epilogue_cl_kernel(const EpiArgs p, unsigned chunks_per_sample, long long items, int cv_shift) {
     using S = typename Acc<T>::type;
     constexpr int N = Vec<T>::N;
@@ -418,19 +430,19 @@ __global__ void __launch_bounds__(256) modconv_epilogue_cl_kernel(const EpiArgs 
                 if (p.noise) t = p.scale ? vx[u][j] * d[j] + nz : vx[u][j] + nz;
                 out[j] = eval<S, A>(t, p.b ? bb[j] : (S)0, (S)0, (S)0, (S)1, 0, alpha, gain, clamp);
             }
-            if (p.y) store_vec((T*)p.y, vbase + vi, out);
+            if (p.y) store_vec((TO*)p.y, vbase + vi, out);
             if (p.y2) {
                 S d2[N];
                 load_vec_keep<T>((const T*)p.scale2, (long long)smp * cv + c0, d2);
 #pragma unroll
                 for (int j = 0; j < N; ++j) out[j] *= d2[j];
-                store_vec((T*)p.y2, vbase + vi, out);
+                store_vec((TO*)p.y2, vbase + vi, out);
             }
         }
     }
 }
 
-template <typename T, int A>
+template <typename T, typename TO, int A>
 static int launch_epilogue(const EpiArgs& p, int channels_last, cudaStream_t st) {
     constexpr int UNROLL = 4;
     constexpr int N = Vec<T>::N;
@@ -445,10 +457,11 @@ static int launch_epilogue(const EpiArgs& p, int channels_last, cudaStream_t st)
         const long long cvn = p.c / N;
         int cv_shift = -1;
         if ((cvn & (cvn - 1)) == 0) { cv_shift = 0; while ((1ll << cv_shift) < cvn) ++cv_shift; }
-        modconv_epilogue_cl_kernel<T, A, UNROLL><<<(unsigned)blocks, 256, 0, st>>>(p, (unsigned)cps, items, cv_shift);
+        modconv_epilogue_cl_kernel<T, TO, A, UNROLL><<<(unsigned)blocks, 256, 0, st>>>(p, (unsigned)cps, items, cv_shift);
         IDE3D_CHECK_LAUNCH("modconv_epilogue_cl_kernel");
         return IDE3D_OK;
     }
+    if constexpr (!std::is_same<T, TO>::value) IDE3D_FAIL(IDE3D_UNSUPPORTED, "modconv_epilogue: a separate output dtype needs channels_last");
     if (p.hw % N != 0) IDE3D_FAIL(IDE3D_UNSUPPORTED, "modconv_epilogue: H*W must be a multiple of %d", N);
     const long long cpp = ceil_div<long long>(p.hw / N, 256ll * UNROLL);
     const long long items = p.n * p.c * cpp;
@@ -461,15 +474,15 @@ static int launch_epilogue(const EpiArgs& p, int channels_last, cudaStream_t st)
 template <typename T>
 static int dispatch_epilogue(const EpiArgs& p, int act, int channels_last, cudaStream_t st) {
     switch (act) {
-        case 1: return launch_epilogue<T, 1>(p, channels_last, st);
-        case 2: return launch_epilogue<T, 2>(p, channels_last, st);
-        case 3: return launch_epilogue<T, 3>(p, channels_last, st);
-        case 4: return launch_epilogue<T, 4>(p, channels_last, st);
-        case 5: return launch_epilogue<T, 5>(p, channels_last, st);
-        case 6: return launch_epilogue<T, 6>(p, channels_last, st);
-        case 7: return launch_epilogue<T, 7>(p, channels_last, st);
-        case 8: return launch_epilogue<T, 8>(p, channels_last, st);
-        case 9: return launch_epilogue<T, 9>(p, channels_last, st);
+        case 1: return launch_epilogue<T, T, 1>(p, channels_last, st);
+        case 2: return launch_epilogue<T, T, 2>(p, channels_last, st);
+        case 3: return launch_epilogue<T, T, 3>(p, channels_last, st);
+        case 4: return launch_epilogue<T, T, 4>(p, channels_last, st);
+        case 5: return launch_epilogue<T, T, 5>(p, channels_last, st);
+        case 6: return launch_epilogue<T, T, 6>(p, channels_last, st);
+        case 7: return launch_epilogue<T, T, 7>(p, channels_last, st);
+        case 8: return launch_epilogue<T, T, 8>(p, channels_last, st);
+        case 9: return launch_epilogue<T, T, 9>(p, channels_last, st);
     }
     IDE3D_FAIL(IDE3D_INVALID, "modconv_epilogue: unknown activation index %d", act);
 }
@@ -493,6 +506,10 @@ extern "C" int ide3d_modconv_epilogue(const void* x, const void* scale, const vo
         case IDE3D_F32: return ide3d::dispatch_epilogue<float>(p, act, channels_last, st);
         case IDE3D_F16: return ide3d::dispatch_epilogue<__half>(p, act, channels_last, st);
         case IDE3D_F64: return ide3d::dispatch_epilogue<double>(p, act, channels_last, st);
+        case IDE3D_DTYPE2(IDE3D_F32, IDE3D_F16):                 // the modulation in front of an fp16 convolution: linear / lrelu
+            if (act == 1) return ide3d::launch_epilogue<float, __half, 1>(p, channels_last, st);
+            if (act == 3) return ide3d::launch_epilogue<float, __half, 3>(p, channels_last, st);
+            IDE3D_FAIL(IDE3D_UNSUPPORTED, "modconv_epilogue: fp16 output for linear / lrelu only");
     }
     IDE3D_FAIL(IDE3D_INVALID, "modconv_epilogue: unsupported dtype %d", dtype);
 }
@@ -515,11 +532,12 @@ namespace ide3d {
 constexpr int kRgbMax = 4;
 
 struct EpiRgbArgs {
-    const float *x, *scale, *noise, *b;
+    const void* x;                        // T: float, or __half (the fp16 output of the convolution)
+    const float *scale, *noise, *b;
     const float* yscale;
-    float* y;
+    void* y;                              // T, as x
     const float* scale2;
-    float* y2;
+    void* y2;                             // T, as x
     const float *wrgb, *srgb, *brgb;
     float* rgb;
     float alpha, gain, clamp;
@@ -532,7 +550,7 @@ __device__ __forceinline__ void load4(const float* p, long long v, float (&o)[4]
     o[0] = t.x; o[1] = t.y; o[2] = t.z; o[3] = t.w;
 }
 
-template <int A, bool kShfl>
+template <typename T, int A, bool kShfl>
 __global__ void __launch_bounds__(256) modconv_epilogue_rgb_cl_kernel(const EpiRgbArgs p, int ppb, unsigned chunks_per_sample,
                                                                      long long items) {
     constexpr int UNROLL = 4;
@@ -570,7 +588,7 @@ __global__ void __launch_bounds__(256) modconv_epilogue_rgb_cl_kernel(const EpiR
 #pragma unroll
         for (int u = 0; u < UNROLL; ++u) {
             const unsigned pix = pix0 + u * ppb + lp;
-            if (lane_on && pix < (unsigned)p.hw) load_vec(p.x, vbase + pix * cv + c0, vx[u]);
+            if (lane_on && pix < (unsigned)p.hw) load_vec((const T*)p.x, vbase + pix * cv + c0, vx[u]);
         }
 #pragma unroll
         for (int u = 0; u < UNROLL; ++u) {
@@ -590,12 +608,12 @@ __global__ void __launch_bounds__(256) modconv_epilogue_rgb_cl_kernel(const EpiR
                 if (p.y) {
 #pragma unroll
                     for (int j = 0; j < 4; ++j) out[j] = p.yscale ? t[j] * ys[j] : t[j];
-                    store_vec(p.y, v, out);
+                    store_vec((T*)p.y, v, out);
                 }
                 if (p.y2) {
 #pragma unroll
                     for (int j = 0; j < 4; ++j) out[j] = t[j] * s2[j];
-                    store_vec(p.y2, v, out);
+                    store_vec((T*)p.y2, v, out);
                 }
                 if (want_rgb) {
 #pragma unroll
@@ -631,7 +649,7 @@ __global__ void __launch_bounds__(256) modconv_epilogue_rgb_cl_kernel(const EpiR
     }
 }
 
-template <int A>
+template <typename T, int A>
 static int launch_epilogue_rgb(const EpiRgbArgs& p, cudaStream_t st) {
     constexpr int UNROLL = 4;
     const int cv = p.c / 4;
@@ -641,10 +659,26 @@ static int launch_epilogue_rgb(const EpiRgbArgs& p, cudaStream_t st) {
     const long long items = (long long)p.n * cps;
     const long long cap = (long long)sm_count() * 8;
     const long long blocks = items < cap ? items : cap;
-    if (shfl) modconv_epilogue_rgb_cl_kernel<A, true><<<(unsigned)blocks, 256, 0, st>>>(p, ppb, (unsigned)cps, items);
-    else modconv_epilogue_rgb_cl_kernel<A, false><<<(unsigned)blocks, 256, 0, st>>>(p, ppb, (unsigned)cps, items);
+    if (shfl) modconv_epilogue_rgb_cl_kernel<T, A, true><<<(unsigned)blocks, 256, 0, st>>>(p, ppb, (unsigned)cps, items);
+    else modconv_epilogue_rgb_cl_kernel<T, A, false><<<(unsigned)blocks, 256, 0, st>>>(p, ppb, (unsigned)cps, items);
     IDE3D_CHECK_LAUNCH("modconv_epilogue_rgb_cl_kernel");
     return IDE3D_OK;
+}
+
+template <typename T>
+static int dispatch_epilogue_rgb(const EpiRgbArgs& p, int act, cudaStream_t st) {
+    switch (act) {
+        case 1: return launch_epilogue_rgb<T, 1>(p, st);
+        case 2: return launch_epilogue_rgb<T, 2>(p, st);
+        case 3: return launch_epilogue_rgb<T, 3>(p, st);
+        case 4: return launch_epilogue_rgb<T, 4>(p, st);
+        case 5: return launch_epilogue_rgb<T, 5>(p, st);
+        case 6: return launch_epilogue_rgb<T, 6>(p, st);
+        case 7: return launch_epilogue_rgb<T, 7>(p, st);
+        case 8: return launch_epilogue_rgb<T, 8>(p, st);
+        case 9: return launch_epilogue_rgb<T, 9>(p, st);
+    }
+    IDE3D_FAIL(IDE3D_INVALID, "modconv_epilogue_rgb: unknown activation index %d", act);
 }
 
 }  // namespace ide3d
@@ -666,23 +700,13 @@ extern "C" int ide3d_modconv_epilogue_rgb(const void* x, const void* scale, cons
     IDE3D_REQUIRE((all & 15) == 0, "modconv_epilogue_rgb: x, y, y2 and the per-channel operands must be 16-byte aligned");
     IDE3D_REQUIRE((((uintptr_t)noise | (uintptr_t)wrgb | (uintptr_t)srgb | (uintptr_t)brgb | (uintptr_t)rgb) & 3) == 0,
                   "modconv_epilogue_rgb: noise / ToRGB operands must be 4-byte aligned");
-    if (dtype != IDE3D_F32) IDE3D_FAIL(IDE3D_UNSUPPORTED, "modconv_epilogue_rgb: float32 only");
+    const bool f16 = dtype == IDE3D_DTYPE2(IDE3D_F16, IDE3D_F16);
+    if (dtype != IDE3D_F32 && !f16) IDE3D_FAIL(IDE3D_UNSUPPORTED, "modconv_epilogue_rgb: float32, or fp16 x / y / y2 with float32 operands only");
     if (c % 4 != 0 || c > 512) IDE3D_FAIL(IDE3D_UNSUPPORTED, "modconv_epilogue_rgb: needs C %% 4 == 0 and C <= 512 (got %lld)", (long long)c);
     if (hw * (c / 4) >= (1ll << 31) || n >= (1ll << 31)) IDE3D_FAIL(IDE3D_UNSUPPORTED, "modconv_epilogue_rgb: more than 2^31 vectors per sample");
-    ide3d::EpiRgbArgs p{(const float*)x, (const float*)scale, (const float*)noise, (const float*)b, (const float*)yscale, (float*)y,
-                        (const float*)scale2, (float*)y2, (const float*)wrgb, (const float*)srgb, (const float*)brgb, (float*)rgb,
+    ide3d::EpiRgbArgs p{x, (const float*)scale, (const float*)noise, (const float*)b, (const float*)yscale, y,
+                        (const float*)scale2, y2, (const float*)wrgb, (const float*)srgb, (const float*)brgb, (float*)rgb,
                         alpha, gain, clamp, (int)n, (int)c, (int)hw, rgb ? (int)rgb_channels : 0, (int)noise_batch};
     cudaStream_t st = (cudaStream_t)stream;
-    switch (act) {
-        case 1: return ide3d::launch_epilogue_rgb<1>(p, st);
-        case 2: return ide3d::launch_epilogue_rgb<2>(p, st);
-        case 3: return ide3d::launch_epilogue_rgb<3>(p, st);
-        case 4: return ide3d::launch_epilogue_rgb<4>(p, st);
-        case 5: return ide3d::launch_epilogue_rgb<5>(p, st);
-        case 6: return ide3d::launch_epilogue_rgb<6>(p, st);
-        case 7: return ide3d::launch_epilogue_rgb<7>(p, st);
-        case 8: return ide3d::launch_epilogue_rgb<8>(p, st);
-        case 9: return ide3d::launch_epilogue_rgb<9>(p, st);
-    }
-    IDE3D_FAIL(IDE3D_INVALID, "modconv_epilogue_rgb: unknown activation index %d", act);
+    return f16 ? ide3d::dispatch_epilogue_rgb<__half>(p, act, st) : ide3d::dispatch_epilogue_rgb<float>(p, act, st);
 }

@@ -16,6 +16,8 @@
 #include <cuda.h>
 #include <stdlib.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace ide3d {
@@ -38,7 +40,8 @@ struct UpfirArgs {
     const void* bias = nullptr;
     // ide3d_upfirdn2d_epilogue only (channels_last patch kernel): the modulated-convolution tail applied to the FIR output
     //   v = act(fir * scale[n,c] + noise[(n),oy,ox] + bias[c]) * gain, clamped;  y = v (if y != NULL);  y2 = v * scale2[n,c]
-    int epi = 0, act = 1, noise_batch = 1;
+    //   mixed formats (kMode below): add fp16 with x / y / bias float32; or x / y / y2 fp16 with the tail operands float32
+    int epi = 0, act = 1, noise_batch = 1, mixed = 0;
     float alpha = 0.f, act_gain = 1.f, clamp = -1.f;
     const void *scale = nullptr, *noise = nullptr, *scale2 = nullptr;
     void* y2 = nullptr;
@@ -467,12 +470,21 @@ template <> struct V4<__half> {
     }
 };
 
+// What follows the FIR in the channels_last kernels.  kPlain: nothing, or the skip add with every tensor of type T; kEpi: the
+// modconv tail with its operands of type T; kEpiF32: the tail with float32 operands (scale, noise, bias, scale2) on fp16 x / y / y2;
+// kAddF16: the skip add of an fp16 `add` to float32 x / y / bias.
+enum { kPlain = 0, kEpi = 1, kEpiF32 = 2, kAddF16 = 3 };
+template <typename T, int kMode> using TailT = typename std::conditional<kMode == kEpiF32, float, T>::type;
+template <typename T, int kMode> using AddT = typename std::conditional<kMode == kAddF16, __half, T>::type;
+
 // One 4x4 output patch x 4 channels: accumulate from a window supplied by `load(r, q, out[4])` (global memory with bounds
 // checks, or a TMA-staged shared-memory tile), then the optional skip-add / modconv tail, then the stores.
-template <typename T, int UX, int UY, int DX, int DY, int FW, int FH, int PHX, int PHY, bool kEpi, typename LoadFn>
+template <typename T, int UX, int UY, int DX, int DY, int FW, int FH, int PHX, int PHY, int kMode, typename LoadFn>
 __device__ __forceinline__ void cl_patch_body(const UpfirArgs& p, const float (&fk)[FH][FW], int n, int cv, int ox0, int oy0, LoadFn load) {
     using AX = Axis<UX, DX, FW, PHX>;
     using AY = Axis<UY, DY, FH, PHY>;
+    using TA = AddT<T, kMode>;
+    using TP = TailT<T, kMode>;
     float acc[kPatch][kPatch][4];
 #pragma unroll
     for (int a = 0; a < kPatch; ++a)
@@ -484,7 +496,7 @@ __device__ __forceinline__ void cl_patch_body(const UpfirArgs& p, const float (&
         // skip-connection form (upsample2d(img) + y + b): the accumulators START from the new contribution, so its 16 loads are in
         // flight together with the window loads instead of after the FIR (the kernel is latency bound) -- same registers, twice the
         // loads in flight
-        const T* ain = (const T*)p.add + n * p.asn + cv * 4;
+        const TA* ain = (const TA*)p.add + n * p.asn + cv * 4;
         float bv[4] = {0.f, 0.f, 0.f, 0.f};
         if (p.bias != nullptr) V4<T>::ld((const T*)p.bias + cv * 4, bv);
 #pragma unroll
@@ -493,7 +505,7 @@ __device__ __forceinline__ void cl_patch_body(const UpfirArgs& p, const float (&
             for (int b = 0; b < kPatch; ++b)
                 if (oy0 + a < p.out_h && ox0 + b < p.out_w) {
                     float av[4];
-                    V4<T>::ld(ain + (oy0 + a) * p.ash + (ox0 + b) * p.asw, av);
+                    V4<TA>::ld(ain + (oy0 + a) * p.ash + (ox0 + b) * p.asw, av);
 #pragma unroll
                     for (int c = 0; c < 4; ++c) acc[a][b][c] = av[c] + bv[c];
                 }
@@ -523,12 +535,12 @@ __device__ __forceinline__ void cl_patch_body(const UpfirArgs& p, const float (&
         }
     }
     T* yout = (T*)p.y + n * p.osn + cv * 4;
-    if constexpr (kEpi) {
+    if constexpr (kMode == kEpi || kMode == kEpiF32) {
         float dv[4] = {1.f, 1.f, 1.f, 1.f}, bv[4] = {0.f, 0.f, 0.f, 0.f}, d2[4] = {1.f, 1.f, 1.f, 1.f};
-        if (p.scale != nullptr) V4<T>::ld((const T*)p.scale + (long long)n * p.in_c + cv * 4, dv);
-        if (p.bias != nullptr) V4<T>::ld((const T*)p.bias + cv * 4, bv);
-        if (p.y2 != nullptr) V4<T>::ld((const T*)p.scale2 + (long long)n * p.in_c + cv * 4, d2);
-        const T* nz = (p.noise != nullptr) ? (const T*)p.noise + (p.noise_batch == 1 ? 0ll : (long long)n * p.out_h * p.out_w) : nullptr;
+        if (p.scale != nullptr) V4<TP>::ld((const TP*)p.scale + (long long)n * p.in_c + cv * 4, dv);
+        if (p.bias != nullptr) V4<TP>::ld((const TP*)p.bias + cv * 4, bv);
+        if (p.y2 != nullptr) V4<TP>::ld((const TP*)p.scale2 + (long long)n * p.in_c + cv * 4, d2);
+        const TP* nz = (p.noise != nullptr) ? (const TP*)p.noise + (p.noise_batch == 1 ? 0ll : (long long)n * p.out_h * p.out_w) : nullptr;
         T* y2out = (p.y2 != nullptr) ? (T*)p.y2 + n * p.osn + cv * 4 : nullptr;
 #pragma unroll
         for (int a = 0; a < kPatch; ++a) {
@@ -536,7 +548,7 @@ __device__ __forceinline__ void cl_patch_body(const UpfirArgs& p, const float (&
 #pragma unroll
             for (int b = 0; b < kPatch; ++b) {
                 if (ox0 + b >= p.out_w) continue;
-                const float nv = nz ? ld<T>(nz + (long long)(oy0 + a) * p.out_w + (ox0 + b)) : 0.f;
+                const float nv = nz ? ld<TP>(nz + (long long)(oy0 + a) * p.out_w + (ox0 + b)) : 0.f;
                 float v[4];
 #pragma unroll
                 for (int c = 0; c < 4; ++c) {
@@ -578,7 +590,7 @@ __device__ __forceinline__ void load_filter(const UpfirArgs& p, float (&fk)[FH][
         }
 }
 
-template <typename T, int UX, int UY, int DX, int DY, int FW, int FH, int PHX, int PHY, bool kEpi>
+template <typename T, int UX, int UY, int DX, int DY, int FW, int FH, int PHX, int PHY, int kMode>
 __global__ void __launch_bounds__(256) upfirdn2d_cl_patch_kernel(const UpfirArgs p, int patches_x, int patches_y) {
     using AX = Axis<UX, DX, FW, PHX>;
     using AY = Axis<UY, DY, FH, PHY>;
@@ -601,7 +613,7 @@ __global__ void __launch_bounds__(256) upfirdn2d_cl_patch_kernel(const UpfirArgs
         const int ox0 = pxi * kPatch, oy0 = pyi * kPatch;
         const int ix0 = ox0 * DX / UX - ax + AX::lo(), iy0 = oy0 * DY / UY - ay + AY::lo();
         const T* xin = (const T*)p.x + (long long)n * p.isn + cv * 4;
-        cl_patch_body<T, UX, UY, DX, DY, FW, FH, PHX, PHY, kEpi>(p, fk, n, cv, ox0, oy0, [&](int r, int q, float (&w)[4]) {
+        cl_patch_body<T, UX, UY, DX, DY, FW, FH, PHX, PHY, kMode>(p, fk, n, cv, ox0, oy0, [&](int r, int q, float (&w)[4]) {
             const int gy = iy0 + r, gx = ix0 + q;
             if ((unsigned)gy < (unsigned)p.in_h && (unsigned)gx < (unsigned)p.in_w) V4<T>::ld(xin + gy * p.ish + gx * p.isw, w);
             else { w[0] = 0.f; w[1] = 0.f; w[2] = 0.f; w[3] = 0.f; }
@@ -650,7 +662,7 @@ template <> struct V4s<__half> {
     }
 };
 
-template <typename T, int UX, int UY, int DX, int DY, int FW, int FH, int PHX, int PHY, bool kEpi, int CB>
+template <typename T, int UX, int UY, int DX, int DY, int FW, int FH, int PHX, int PHY, int kMode, int CB>
 __global__ void __launch_bounds__(256, 2) upfirdn2d_cl_tma_kernel(const UpfirArgs p, int tiles_x, int tiles_y, int cblocks,
                                                                const __grid_constant__ CUtensorMap tmap) {
     using GM = ClTmaGeom<T, UX, UY, DX, DY, FW, FH, PHX, PHY, CB>;
@@ -699,7 +711,7 @@ __global__ void __launch_bounds__(256, 2) upfirdn2d_cl_tma_kernel(const UpfirArg
         const T* tile = reinterpret_cast<const T*>(base + cur * GM::kTileBytes) + ((pty * AY::kStep) * GM::BW + ptx * AX::kStep) * kClCB + cvl * 4;
         const int ox0 = ox_t + ptx * kPatch, oy0 = oy_t + pty * kPatch;
         if (ox0 < p.out_w && oy0 < p.out_h)
-            cl_patch_body<T, UX, UY, DX, DY, FW, FH, PHX, PHY, kEpi>(p, fk, n, cb * (kClCB / 4) + cvl, ox0, oy0, [&](int r, int q, float (&w)[4]) {
+            cl_patch_body<T, UX, UY, DX, DY, FW, FH, PHX, PHY, kMode>(p, fk, n, cb * (kClCB / 4) + cvl, ox0, oy0, [&](int r, int q, float (&w)[4]) {
                 V4s<T>::ld(tile + (r * GM::BW + q) * kClCB, w);
             });
         __syncthreads();                                                     // every thread is done with stage `cur`
@@ -721,8 +733,12 @@ static int launch_cl_tma(const UpfirArgs& p, cudaStream_t st_) {
                                       const_cast<void*>(p.x), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                       CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) IDE3D_FAIL(IDE3D_UNSUPPORTED, "upfirdn2d: cuTensorMapEncodeTiled (channels_last) failed (%d)", (int)r);
-    void (*kern)(const UpfirArgs, int, int, int, const CUtensorMap) = p.epi ? upfirdn2d_cl_tma_kernel<T, UX, UY, DX, DY, FW, FH, PHX, PHY, true, CB>
-                                                                            : upfirdn2d_cl_tma_kernel<T, UX, UY, DX, DY, FW, FH, PHX, PHY, false, CB>;
+    void (*kern)(const UpfirArgs, int, int, int, const CUtensorMap) = p.epi ? upfirdn2d_cl_tma_kernel<T, UX, UY, DX, DY, FW, FH, PHX, PHY, kEpi, CB>
+                                                                            : upfirdn2d_cl_tma_kernel<T, UX, UY, DX, DY, FW, FH, PHX, PHY, kPlain, CB>;
+    if constexpr (std::is_same<T, __half>::value)
+        if (p.mixed) kern = upfirdn2d_cl_tma_kernel<T, UX, UY, DX, DY, FW, FH, PHX, PHY, kEpiF32, CB>;
+    if constexpr (std::is_same<T, float>::value)
+        if (p.mixed) return IDE3D_UNSUPPORTED;                                  // the fp16 skip add runs in the L1-gather kernel
     const size_t smem = GM::kSmem;
     if (smem > 48 * 1024) IDE3D_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int tiles_x = ceil_div(p.out_w, kClTileW), tiles_y = ceil_div(p.out_h, kClTileH), cblocks = p.in_c / kClCB;
@@ -763,8 +779,13 @@ static int launch_cl_patch(const UpfirArgs& p, cudaStream_t st_) {
     long long grid = ceil_div<long long>(total, 256);
     const long long cap = (long long)sm_count() * 8;
     if (grid > cap) grid = cap;
-    if (p.epi) upfirdn2d_cl_patch_kernel<T, UX, UY, DX, DY, FW, FH, PHX, PHY, true><<<(unsigned)grid, 256, 0, st_>>>(p, patches_x, patches_y);
-    else upfirdn2d_cl_patch_kernel<T, UX, UY, DX, DY, FW, FH, PHX, PHY, false><<<(unsigned)grid, 256, 0, st_>>>(p, patches_x, patches_y);
+    void (*kern)(const UpfirArgs, int, int) = p.epi ? upfirdn2d_cl_patch_kernel<T, UX, UY, DX, DY, FW, FH, PHX, PHY, kEpi>
+                                                    : upfirdn2d_cl_patch_kernel<T, UX, UY, DX, DY, FW, FH, PHX, PHY, kPlain>;
+    if constexpr (std::is_same<T, __half>::value)
+        if (p.mixed) kern = upfirdn2d_cl_patch_kernel<T, UX, UY, DX, DY, FW, FH, PHX, PHY, kEpiF32>;
+    if constexpr (std::is_same<T, float>::value)
+        if (p.mixed) kern = upfirdn2d_cl_patch_kernel<T, UX, UY, DX, DY, FW, FH, PHX, PHY, kAddF16>;
+    kern<<<(unsigned)grid, 256, 0, st_>>>(p, patches_x, patches_y);
     IDE3D_CHECK_LAUNCH("upfirdn2d_cl_patch_kernel");
     return IDE3D_OK;
 }
@@ -904,16 +925,21 @@ static int upfirdn2d_entry(const ide3d_upfirdn2d_params* q, const void* add, int
     p.fw = q->f_w; p.fh = q->f_h; p.fsw = q->f_stride_w; p.fsh = q->f_stride_h;
     p.out_w = q->out_w; p.out_h = q->out_h;
     p.osw = q->out_stride_w; p.osh = q->out_stride_h; p.osc = q->out_stride_c; p.osn = q->out_stride_n;
+    // mixed formats: fp16 add on float32 x / y (the skip add), or fp16 x / y / y2 with a float32 tail (the FIR epilogue)
+    const int add_mixed = IDE3D_DTYPE2(IDE3D_F32, IDE3D_F16), epi_mixed = IDE3D_DTYPE2(IDE3D_F16, IDE3D_F16);
+    IDE3D_REQUIRE((q->dtype != add_mixed || add != nullptr) && (q->dtype != epi_mixed || e != nullptr),
+                  "upfirdn2d: dtype %d is only defined for the skip add / the epilogue", q->dtype);
+    p.mixed = q->dtype == add_mixed || q->dtype == epi_mixed;
     if (add != nullptr) {
-        const uintptr_t vb = (q->dtype == IDE3D_F16) ? 8 : 16;
-        IDE3D_REQUIRE(((uintptr_t)add % vb) == 0 && (bias == nullptr || ((uintptr_t)bias % vb) == 0) && (asn | ash | asw) % 4 == 0,
+        const uintptr_t vb = (q->dtype == IDE3D_F16) ? 8 : 16, va = (q->dtype == IDE3D_F16 || p.mixed) ? 8 : 16;
+        IDE3D_REQUIRE(((uintptr_t)add % va) == 0 && (bias == nullptr || ((uintptr_t)bias % vb) == 0) && (asn | ash | asw) % 4 == 0,
                       "upfirdn2d_add: add / bias must be aligned to one 4-channel vector");
         p.add = add; p.asn = asn; p.ash = ash; p.asw = asw; p.bias = bias;
     }
     if (e != nullptr) {
-        const uintptr_t vb = (q->dtype == IDE3D_F16) ? 8 : 16;
-        const uintptr_t all = (uintptr_t)e->scale | (uintptr_t)e->b | (uintptr_t)e->scale2 | (uintptr_t)e->y2;
-        IDE3D_REQUIRE(all % vb == 0, "upfirdn2d_epilogue: scale / b / scale2 / y2 must be aligned to one 4-channel vector");
+        const uintptr_t vb = (q->dtype == IDE3D_F16) ? 8 : 16, vy = (q->dtype == IDE3D_F16 || p.mixed) ? 8 : 16;
+        const uintptr_t all = (uintptr_t)e->scale | (uintptr_t)e->b | (uintptr_t)e->scale2;
+        IDE3D_REQUIRE(all % vb == 0 && (uintptr_t)e->y2 % vy == 0, "upfirdn2d_epilogue: scale / b / scale2 / y2 must be aligned to one 4-channel vector");
         IDE3D_REQUIRE((e->y2 == nullptr) == (e->scale2 == nullptr), "upfirdn2d_epilogue: scale2 and y2 go together");
         IDE3D_REQUIRE(e->noise == nullptr || e->noise_batch == 1 || e->noise_batch == q->in_n, "upfirdn2d_epilogue: noise batch must be 1 or n");
         if (e->act != 1 && e->act != 3) IDE3D_FAIL(IDE3D_UNSUPPORTED, "upfirdn2d_epilogue: only linear / lrelu are fused");
@@ -923,7 +949,9 @@ static int upfirdn2d_entry(const ide3d_upfirdn2d_params* q, const void* add, int
     }
     cudaStream_t s = (cudaStream_t)stream;
     switch (q->dtype) {
+        case IDE3D_DTYPE2(IDE3D_F32, IDE3D_F16):
         case IDE3D_F32: return dispatch_upfirdn2d<float>(p, s);
+        case IDE3D_DTYPE2(IDE3D_F16, IDE3D_F16):
         case IDE3D_F16: return dispatch_upfirdn2d<__half>(p, s);
         case IDE3D_F64: return dispatch_upfirdn2d<double>(p, s);
     }

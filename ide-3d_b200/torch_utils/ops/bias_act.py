@@ -133,7 +133,7 @@ def bias_act(x, b=None, dim=1, act='linear', alpha=None, gain=None, clamp=None, 
 
 
 def scaled_bias_act(x, scale=None, noise=None, b=None, act='linear', alpha=None, gain=None, clamp=None, next_scale=None,
-                    only_next=False, emit_y=True, y_scale=None, rgb=None):
+                    only_next=False, emit_y=True, y_scale=None, rgb=None, out_dtype=None, fp32_tail=False):
     """Extension: ``bias_act(fma(x, scale[:, :, None, None], noise), b, act=...)`` -- the tail of an activation-scaled
     modulated convolution (inversion/networks.py:104-105 then :512) -- as ONE sm_90a pass when nothing needs a gradient;
     otherwise exactly that composition of the two reference ops (so autograd behaves as in the reference).
@@ -143,21 +143,30 @@ def scaled_bias_act(x, scale=None, noise=None, b=None, act='linear', alpha=None,
     Further consumers folded into the same pass: emit_y=False drops y (as only_next), y_scale [N,C] returns ``y * y_scale``
     in place of y (the next block's first modulation), rgb=(weight [O,C,1,1], styles [N,C], bias [O] | None) adds the ToRGB
     output ``conv1x1(y * styles, weight) + bias`` as a dense NCHW tensor (ToRGBLayer, :700-707).  With any of these the
-    result is the list of the requested outputs in the order (y, y2, rgb)."""
+    result is the list of the requested outputs in the order (y, y2, rgb).
+    out_dtype=torch.float16 (float32 x, without the folded consumers): y / y2 rounded once to fp16 -- the input of an fp16
+    convolution.  fp32_tail (float16 x, the output of such a convolution, with folded consumers): scale, noise, b and the
+    styles stay float32 and so does the arithmetic; y / y2 are fp16, each rounded once."""
     from . import fma
     if x.device.type != 'cuda':
         raise RuntimeError('ide3d_b200.scaled_bias_act: x must be a CUDA tensor (no CPU path in this package)')
     _init()
     if rgb is not None or y_scale is not None or not emit_y:
-        return _scaled_bias_act_fold(x, scale, noise, b, act, alpha, gain, clamp, next_scale, emit_y and not only_next, y_scale, rgb)
+        assert out_dtype is None
+        return _scaled_bias_act_fold(x, scale, noise, b, act, alpha, gain, clamp, next_scale, emit_y and not only_next, y_scale, rgb,
+                                     fp32_tail)
+    assert not fp32_tail, 'fp32_tail needs a folded consumer (y_scale, rgb or emit_y=False)'
     spec = activation_funcs[act]
     needs_grad = torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (x, scale, noise, b, next_scale))
     if not needs_grad and x.ndim == 4:
         out = _plugin.modconv_epilogue(_layout(x), scale, noise, b, spec.cuda_idx, float(alpha if alpha is not None else spec.def_alpha),
                                        float(gain if gain is not None else spec.def_gain), float(clamp if clamp is not None else -1),
-                                       next_scale=next_scale, only_next=only_next)
+                                       next_scale=next_scale, only_next=only_next, out_dtype=out_dtype)
         if out is not None:
             return out
+    if out_dtype is not None and out_dtype != x.dtype:
+        out = scaled_bias_act(x, scale, noise, b, act=act, alpha=alpha, gain=gain, clamp=clamp, next_scale=next_scale, only_next=only_next)
+        return out.to(out_dtype) if isinstance(out, torch.Tensor) else tuple(t.to(out_dtype) for t in out)
     if scale is not None and noise is not None:
         x = fma.fma(x, scale.to(x.dtype).reshape(x.shape[0], -1, 1, 1), noise.to(x.dtype))
     elif scale is not None:
@@ -171,8 +180,8 @@ def scaled_bias_act(x, scale=None, noise=None, b=None, act='linear', alpha=None,
     return y2 if only_next else (y, y2)
 
 
-def _scaled_bias_act_fold(x, scale, noise, b, act, alpha, gain, clamp, next_scale, emit_y, y_scale, rgb):
-    """`scaled_bias_act` with its consumers folded in: one `ide3d_modconv_epilogue_rgb` pass for channels_last float32 inference;
+def _scaled_bias_act_fold(x, scale, noise, b, act, alpha, gain, clamp, next_scale, emit_y, y_scale, rgb, fp32_tail=False):
+    """`scaled_bias_act` with its consumers folded in: one `ide3d_modconv_epilogue_rgb` pass for channels_last float32 / float16 x;
     for anything else (gradients, other layouts / dtypes / widths) today's composition -- the epilogue, the products with the
     styles and, for rgb, the cuDNN 1x1 convolution followed by the bias."""
     from . import conv2d_resample
@@ -183,9 +192,13 @@ def _scaled_bias_act_fold(x, scale, noise, b, act, alpha, gain, clamp, next_scal
     needs_grad = torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (x, scale, noise, b, next_scale, y_scale, *(rgb or ())))
     if not needs_grad and x.ndim == 4:
         out = _plugin.modconv_epilogue_rgb(x, scale, noise, b, spec.cuda_idx, alpha, gain, clamp_f, emit_y=emit_y, y_scale=y_scale,
-                                           next_scale=next_scale, rgb=rgb)
+                                           next_scale=next_scale, rgb=rgb, fp32_tail=fp32_tail)
         if out is not None:
             return out
+    if fp32_tail and x.dtype != torch.float32:              # the same tail composed in float32, fp16 outputs rounded once
+        out = _scaled_bias_act_fold(x.float(), scale, noise, b, act, alpha, gain, clamp, next_scale, emit_y, y_scale, rgb)
+        n_x = int(emit_y) + int(next_scale is not None)
+        return [t.to(x.dtype) if i < n_x else t for i, t in enumerate(out)]
     y = scaled_bias_act(x, scale, noise, b, act=act, alpha=alpha, gain=gain, clamp=clamp)
     mod = lambda s: y * s.to(y.dtype).reshape(y.shape[0], -1, 1, 1)
     out = []

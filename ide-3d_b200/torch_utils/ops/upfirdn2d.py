@@ -148,11 +148,13 @@ def upsample2d(x, f, up=2, padding=0, flip_filter=False, gain=1, impl='cuda'):
 
 
 def upfirdn2d_epilogue(x, f, padding=0, gain=1, flip_filter=False, scale=None, noise=None, b=None, act='linear', alpha=None,
-                       act_gain=None, clamp=None, next_scale=None, only_next=False):
+                       act_gain=None, clamp=None, next_scale=None, only_next=False, fp32_tail=False):
     """Extension: ``bias_act.scaled_bias_act(upfirdn2d(x, f, padding=padding, gain=gain), scale, noise, b, ...)`` -- what
     follows the transposed convolution of an up=2 SynthesisLayer (conv2d_resample.py:125; inversion/networks.py:104-105, :512)
     -- as one pass when x is channels_last (C % 4 == 0), f is the 4x4 filter and nothing needs a gradient; otherwise that
-    composition.  Returns y, (y, y_next) or y_next like `scaled_bias_act`."""
+    composition.  Returns y, (y, y_next) or y_next like `scaled_bias_act`.
+    fp32_tail (float16 x, the output of an fp16 convolution): the FIR and the tail run in float32 with float32 scale / noise / b /
+    next_scale; the outputs are fp16, each rounded once."""
     from . import bias_act
     if x.device.type != 'cuda':
         raise RuntimeError('ide3d_b200.upfirdn2d_epilogue: x must be a CUDA tensor (no CPU path in this package)')
@@ -163,25 +165,25 @@ def upfirdn2d_epilogue(x, f, padding=0, gain=1, flip_filter=False, scale=None, n
         px0, px1, py0, py1 = _parse_padding(padding)
         e = dict(scale=scale, noise=noise, b=b, act=spec.cuda_idx, alpha=float(alpha if alpha is not None else spec.def_alpha),
                  gain=float(act_gain if act_gain is not None else spec.def_gain), clamp=float(clamp if clamp is not None else -1),
-                 next_scale=next_scale, only_next=only_next)
+                 next_scale=next_scale, only_next=only_next, fp32_tail=fp32_tail)
         out = _plugin.upfirdn2d(x, f.to(x.device), 1, 1, 1, 1, px0, px1, py0, py1, bool(flip_filter), float(gain), epilogue=e)
         if out is not None:
             return out
-    y = upfirdn2d(x, f, padding=padding, gain=gain, flip_filter=flip_filter)
+    y = upfirdn2d(x.float() if fp32_tail else x, f, padding=padding, gain=gain, flip_filter=flip_filter)
     return bias_act.scaled_bias_act(y, scale=scale, noise=noise, b=b, act=act, alpha=alpha, gain=act_gain, clamp=clamp,
-                                    next_scale=next_scale, only_next=only_next)
+                                    next_scale=next_scale, only_next=only_next, out_dtype=x.dtype if fp32_tail else None)
 
 
 def upsample2d_add(x, f, y, b=None, up=2):
     """Extension: ``upsample2d(x, f, up) + y + b[None, :, None, None]`` -- the skip-connection step of a 'skip' synthesis
     block (inversion/networks.py:841-844, with the ToRGB bias of :707 folded in).  One pass when x is channels_last with
     C % 4 == 0, f is the 2-D 4x4 filter, y has stride_c == 1 and nothing needs a gradient; otherwise the composition of the
-    reference ops (``y`` is then not modified)."""
+    reference ops (``y`` is then not modified).  y may be float16 on float32 x (the output of an fp16 1x1 convolution)."""
     if x.device.type != 'cuda':
         raise RuntimeError('ide3d_b200.upsample2d_add: x must be a CUDA tensor (no CPU path in this package)')
     _init()
     needs_grad = torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (x, y, b))
-    if not needs_grad and f is not None and f.ndim == 2 and y.dtype == x.dtype:
+    if not needs_grad and f is not None and f.ndim == 2 and (y.dtype == x.dtype or (y.dtype == torch.float16 and x.dtype == torch.float32)):
         upx, upy = _parse_scaling(up)
         fw, fh = _get_filter_size(f)
         p = [(fw + upx - 1) // 2, (fw - upx) // 2, (fh + upy - 1) // 2, (fh - upy) // 2]

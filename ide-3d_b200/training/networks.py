@@ -9,6 +9,7 @@ Every convolution goes to cuDNN (conv2d_resample -> conv2d_gradfix); the surroun
 sm_90a kernels: upfirdn2d (FIR after the transposed conv, skip-image upsampling) and bias_act.
 """
 
+import math
 import os
 
 import numpy as np
@@ -38,6 +39,37 @@ FUSED_TORGB = os.environ.get('IDE3D_FUSED_TORGB', '1') != '0'
 CONV1X1_AS_MATMUL = os.environ.get('IDE3D_CONV1X1_MM', '0') != '0'
 
 
+def fp16_operands(blocks, force_fp32=False, fused_modconv=None):
+    """Do the convolutions of a chained synthesis call run on fp16 operands (DESIGN.md §2)?  Exactly when cuDNN may use TF32
+    (torch.backends.cudnn.allow_tf32: every operand is then rounded to a 10-bit mantissa anyway, which is what fp16 keeps), the
+    caller did not ask for fp32 (force_fp32) or the grouped convolution, and every block can fold its neighbours' passes into its
+    epilogues (can_fold: NHWC, no conv_clamp) without a use_fp16 block.  The caller also needs the style plan, i.e. fp32 inference
+    without gradients.  The convolution operands are then fp16 -- each tensor between two convolutions is written in fp16 by the
+    epilogue that produces it -- and everything else (styles, demodulation, noise, bias, the epilogues' arithmetic, the ToRGB
+    output and the skip images) stays float32."""
+    return (bool(torch.backends.cudnn.allow_tf32) and not force_fp32 and not fused_modconv
+            and all(b.can_fold() and not b.use_fp16 for b in blocks))
+
+
+def _cached(module, name, tensors, make):
+    """Derived constant of parameters / buffers, recomputed when any of them changes (data pointer, version, device)."""
+    key = tuple((t.data_ptr(), t._version, str(t.device)) for t in tensors)
+    store = module.__dict__.setdefault('_const_cache', {})
+    hit = store.get(name)
+    if hit is None or hit[0] != key:
+        with torch.no_grad():
+            hit = store[name] = (key, make())
+    return hit[1]
+
+
+def _fp16_copy(weight, e=0, transpose=False):
+    """weight * 2^-e (exact) rounded to fp16, in the layout cuDNN's NHWC kernels want; transpose: the [I, O, k, k] operand of the
+    transposed convolution."""
+    fmt = torch.channels_last if CHANNELS_LAST else torch.contiguous_format
+    w = weight.detach().to(torch.float32) * (2.0 ** -e)
+    return (w.transpose(0, 1) if transpose else w).to(torch.float16).contiguous(memory_format=fmt)
+
+
 def _conv1x1_nhwc(x, weight):
     """x [N,I,H,W] channels_last dense, weight [O,I,1,1] -> [N,O,H,W] channels_last (a view of the [N*H*W, O] product)."""
     n, c, h, w = x.shape
@@ -56,15 +88,17 @@ def normalize_2nd_moment(x, dim=1, eps=1e-8):
 
 
 def modulated_conv2d(x, weight, styles, noise=None, up=1, down=1, padding=0, resample_filter=None, demodulate=True,
-                     flip_weight=True, fused_modconv=True, epilogue=None, premodulated=False, dcoefs=None, w_transposed=None):
+                     flip_weight=True, fused_modconv=True, epilogue=None, premodulated=False, dcoefs=None, w_transposed=None, w16=None):
     """Style-modulated convolution (inversion/networks.py:55-130).  x [N,I,H,W], weight [O,I,k,k], styles [N,I].
     epilogue (activation-scaled path only): dict(b, act, gain, clamp) -- the bias_act that always follows (:512, :707) is
     then applied here, fused with the demodulation / noise pass (`bias_act.scaled_bias_act`); optional keys next_scale /
     only_next make that pass also emit `y * next_styles`, the input of the next activation-scaled convolution.
-    premodulated: x already carries `* styles` (written by the previous layer's epilogue)."""
+    premodulated: x already carries `* styles` (written by the previous layer's epilogue).
+    w16 (activation-scaled inference, see fp16_operands): the layer's fp16 weight W * 2^-e (for up > 1 with w_transposed its
+    transposed fp16 copy); the convolution then runs on fp16 operands and dcoefs already carry the 2^e."""
     batch_size = x.shape[0]
     out_channels, in_channels, kh, kw = weight.shape
-    if x.dtype == torch.float16 and demodulate:      # keep fp16 in range (:78-81)
+    if x.dtype == torch.float16 and demodulate and w16 is None:      # keep fp16 in range (:78-81)
         weight = weight * (1 / np.sqrt(in_channels * kh * kw) / weight.norm(float('inf'), dim=[1, 2, 3], keepdim=True))
         styles = styles / styles.norm(float('inf'), dim=1, keepdim=True)
     w = None
@@ -81,23 +115,26 @@ def modulated_conv2d(x, weight, styles, noise=None, up=1, down=1, padding=0, res
         # materialising the [N,O,I,k,k] modulated weight just to reduce it (same value up to fp32 summation order)
         dcoefs = (styles.square() @ weight.square().sum(dim=[2, 3]).t() + 1e-8).rsqrt()
 
-    assert not (premodulated and (fused_modconv or (x.dtype == torch.float16 and demodulate)))
+    assert not (premodulated and (fused_modconv or (x.dtype == torch.float16 and demodulate and w16 is None)))
+    assert w16 is None or not fused_modconv
     if not fused_modconv:                           # scale activations instead of weights (:97-111)
         if not premodulated:
-            x = bias_act.scaled_bias_act(x, scale=styles)       # x * styles[:, :, None, None]
+            x = bias_act.scaled_bias_act(x, scale=styles, **({} if w16 is None else dict(out_dtype=torch.float16)))  # x * styles[:, :, None, None]
+        wc = weight.to(x.dtype) if w16 is None else w16
+        if epilogue is not None and w16 is not None:
+            epilogue = dict(epilogue, fp32_tail=True)                      # fp16 convolution output, float32 tail operands
         if epilogue is not None and up > 1 and down == 1 and kh > 1:      # the FIR after the transposed conv applies the tail
             e = dict(epilogue)
             e['act_gain'] = e.pop('gain', None)
             e.update(scale=dcoefs if demodulate else None, noise=noise)
-            return conv2d_resample.conv2d_resample(x=x, w=weight.to(x.dtype), f=resample_filter, up=up, down=down,
+            return conv2d_resample.conv2d_resample(x=x, w=wc, f=resample_filter, up=up, down=down,
                                                    padding=padding, flip_weight=flip_weight, fir_epilogue=e, w_transposed=w_transposed)
         if (CONV1X1_AS_MATMUL and kh == 1 and kw == 1 and up == 1 and down == 1 and padding == 0 and x.dtype == torch.float32 and x.is_cuda
                 and x.is_contiguous(memory_format=torch.channels_last) and not x.is_contiguous()
                 and not (torch.is_grad_enabled() and (x.requires_grad or weight.requires_grad))):
             x = _conv1x1_nhwc(x, weight)
         else:
-            x = conv2d_resample.conv2d_resample(x=x, w=weight.to(x.dtype), f=resample_filter, up=up, down=down,
-                                                padding=padding, flip_weight=flip_weight)
+            x = conv2d_resample.conv2d_resample(x=x, w=wc, f=resample_filter, up=up, down=down, padding=padding, flip_weight=flip_weight)
         if epilogue is not None:
             return bias_act.scaled_bias_act(x, scale=dcoefs if demodulate else None, noise=noise, **epilogue)
         if demodulate and noise is not None:
@@ -222,11 +259,13 @@ class SynthesisLayer(torch.nn.Module):
         self.bias = torch.nn.Parameter(torch.zeros([out_channels]))
 
     def forward(self, x, w, noise_mode='random', fused_modconv=True, gain=1, styles=None, premodulated=False, next_styles=None,
-                only_next=False, dcoefs=None, y_styles=None, emit_y=True, rgb=None):
+                only_next=False, dcoefs=None, y_styles=None, emit_y=True, rgb=None, fp16=False):
         """styles / premodulated / next_styles / only_next: block-internal chaining of activation-scaled layers -- the
         epilogue of this layer can already write `y * next_styles` for the layer that follows (see SynthesisBlock._features).
         y_styles / emit_y / rgb (3x3 layers without upsampling): the epilogue returns `y * y_styles` in place of y, or no y,
-        and the ToRGB output of rgb = (weight, styles, bias) -- `bias_act.scaled_bias_act`."""
+        and the ToRGB output of rgb = (weight, styles, bias) -- `bias_act.scaled_bias_act`.
+        fp16 (inference on the chained path, see fp16_operands): the convolution runs on fp16 operands with the weight copy
+        W * 2^-fp16_exponent(); dcoefs must then carry the factor 2^fp16_exponent() (StylePlan.run(fp16_blocks=...) does)."""
         assert noise_mode in ['random', 'const', 'none']
         if styles is None:
             styles = self.affine(w)
@@ -251,23 +290,33 @@ class SynthesisLayer(torch.nn.Module):
             epilogue['emit_y'] = False
         if rgb is not None:
             epilogue['rgb'] = rgb
-        w_t = None
-        if inference and self.up > 1 and not fused_modconv and x.dtype == self.weight.dtype:
+        w_t = w16 = None
+        if fp16:
+            assert inference and not fused_modconv and dcoefs is not None
+            e = self.fp16_exponent()
+            if self.up > 1:
+                w_t = w16 = self._cached('w_t16', (self.weight,), lambda: _fp16_copy(self.weight, e, transpose=True))
+            else:
+                w16 = self._cached('w16', (self.weight,), lambda: _fp16_copy(self.weight, e))
+        elif inference and self.up > 1 and not fused_modconv and x.dtype == self.weight.dtype:
             fmt = torch.channels_last if CHANNELS_LAST else torch.contiguous_format
             w_t = self._cached('w_t', (self.weight,), lambda: self.weight.detach().transpose(0, 1).contiguous(memory_format=fmt))
         return modulated_conv2d(x=x, weight=self.weight, styles=styles, noise=noise, up=self.up, padding=self.padding,
                                 resample_filter=self.resample_filter, flip_weight=(self.up == 1), fused_modconv=fused_modconv,
-                                epilogue=epilogue, premodulated=premodulated, dcoefs=None if fused_modconv else dcoefs, w_transposed=w_t)
+                                epilogue=epilogue, premodulated=premodulated, dcoefs=None if fused_modconv else dcoefs, w_transposed=w_t,
+                                w16=w16)
 
-    def _cached(self, name, tensors, make):
-        """Derived constant of parameters / buffers, recomputed when any of them changes (data pointer, version, device)."""
-        key = tuple((t.data_ptr(), t._version, str(t.device)) for t in tensors)
-        store = self.__dict__.setdefault('_const_cache', {})
-        hit = store.get(name)
-        if hit is None or hit[0] != key:
-            with torch.no_grad():
-                hit = store[name] = (key, make())
-        return hit[1]
+    def fp16_exponent(self):
+        """e of the fp16 weight copy W * 2^-e: round(log2(sqrt(fan_in) * rms(W))), so that the convolution output before
+        demodulation keeps the magnitude of its input `x * styles`, far from fp16's 65504.  Powers of two scale exactly: the
+        demodulation coefficient takes 2^e back in float32 and no rounding changes."""
+        def make():
+            w = self.weight.detach().to(torch.float32)
+            rms = float(w.square().mean().sqrt())
+            return int(round(math.log2(math.sqrt(w[0].numel()) * rms))) if rms > 0 else 0
+        return self._cached('fp16_e', (self.weight,), make)
+
+    _cached = _cached
 
 
 @persistence.persistent_class
@@ -287,9 +336,16 @@ class ToRGBLayer(torch.nn.Module):
         return self.affine(w) * self.weight_gain
 
     def forward(self, x, w, fused_modconv=True, styles=None, premodulated=False, raw=False):
-        """raw: return the convolution output WITHOUT the bias (the caller folds `self.bias` into the skip-connection pass)."""
+        """raw: return the convolution output WITHOUT the bias (the caller folds `self.bias` into the skip-connection pass).
+        An fp16 premodulated x (the fp16 operand path, see fp16_operands) is convolved with the layer's fp16 weight copy; the
+        output is fp16, or float32 with the bias added.  The styles already carry 1/sqrt(fan_in) (weight_gain), so the output has
+        the magnitude of x * rms(W) and the copy is not rescaled (e = 0)."""
         if styles is None:
             styles = self.styles(w)
+        if premodulated and x.dtype == torch.float16 and self.weight.dtype == torch.float32:
+            w16 = _cached(self, 'w16', (self.weight,), lambda: _fp16_copy(self.weight))
+            y = modulated_conv2d(x=x, weight=self.weight, styles=styles, demodulate=False, fused_modconv=False, premodulated=True, w16=w16)
+            return y if raw else bias_act.bias_act(y.to(torch.float32), self.bias, clamp=self.conv_clamp)
         return modulated_conv2d(x=x, weight=self.weight, styles=styles, demodulate=False, fused_modconv=fused_modconv,
                                 epilogue=None if raw else dict(b=self.bias, clamp=self.conv_clamp), premodulated=premodulated)
 
@@ -334,11 +390,13 @@ class SynthesisBlock(torch.nn.Module):
         """-> (x, w_rgb, fused_modconv, rgb_in, y_rgb).  Keys of layer_kwargs a synthesis network uses to chain its blocks (each
         needs the chained path below): premodulated_x -- x already carries conv0's styles (the previous block's epilogue wrote
         them); x_next_styles [N, C] -- return `x * x_next_styles` (the next block's conv0 styles) instead of x; drop_x -- return
-        no x (nothing consumes it).  y_rgb is the ToRGB output (bias included) when conv1's epilogue computed it."""
+        no x (nothing consumes it); fp16_operands -- run the convolutions on fp16 operands (fp16_operands(); needs the style plan's
+        dcoefs for that path).  y_rgb is the ToRGB output (bias included) when conv1's epilogue computed it."""
         layer_kwargs = dict(layer_kwargs)
         premod_in = layer_kwargs.pop('premodulated_x', False)
         x_next_styles = layer_kwargs.pop('x_next_styles', None)
         drop_x = layer_kwargs.pop('drop_x', False)
+        fp16 = layer_kwargs.pop('fp16_operands', False)
         misc.assert_shape(ws, [None, self.num_conv + self.num_torgb, self.w_dim])
         w_iter = iter(ws.unbind(dim=1))
         dtype = torch.float16 if self.use_fp16 and not force_fp32 else torch.float32
@@ -356,13 +414,15 @@ class SynthesisBlock(torch.nn.Module):
             ws.requires_grad or any(p.requires_grad for p in self.parameters())))
         if not chain and (premod_in or x_next_styles is not None or drop_x):
             raise RuntimeError('SynthesisBlock: cross-block chaining needs the chained fp32 inference path')
+        if fp16 and not (chain and self.can_fold() and 'style_plan' in layer_kwargs):
+            raise RuntimeError('SynthesisBlock: fp16 operands need the chained inference path with a style plan')
         rgb_in = y_rgb = None
         if self.in_channels == 0:
             x = self.const.to(dtype=dtype).unsqueeze(0).repeat([ws.shape[0], 1, 1, 1]).contiguous(memory_format=memory_format)
             w1 = next(w_iter)
         else:
             misc.assert_shape(x, [None, self.in_channels, self.resolution // 2, self.resolution // 2])
-            x = x.to(dtype=dtype, memory_format=memory_format)
+            x = x.to(memory_format=memory_format) if fp16 else x.to(dtype=dtype, memory_format=memory_format)   # fp16: x * s0 in fp16
             w0, w1 = next(w_iter), next(w_iter)
         w_rgb = next(w_iter)
         plan = layer_kwargs.pop('style_plan', None) if chain else None
@@ -376,7 +436,7 @@ class SynthesisBlock(torch.nn.Module):
             pre = False
             if self.in_channels != 0:
                 x = self.conv0(x, w0, fused_modconv=False, styles=s0, dcoefs=d0, premodulated=premod_in, next_styles=s1, only_next=True,
-                               **layer_kwargs)
+                               fp16=fp16, **layer_kwargs)
                 pre = True
             # ToRGB of <= 4 channels inside conv1's epilogue: a 3 x C dot product per pixel instead of x * s_rgb + a 1x1 convolution
             fold_rgb = x.is_cuda and self.torgb.weight.shape[0] <= 4 and self.can_fold()
@@ -388,7 +448,7 @@ class SynthesisBlock(torch.nn.Module):
             if fold_rgb:
                 fold['rgb'] = (self.torgb.weight, s_rgb, self.torgb.bias)
             outs = self.conv1(x, w1, fused_modconv=False, styles=s1, dcoefs=d1, premodulated=pre, next_styles=None if fold_rgb else s_rgb,
-                              **fold, **layer_kwargs)          # (y | y * y_styles)?, (y * s_rgb | ToRGB output)
+                              fp16=fp16, **fold, **layer_kwargs)          # (y | y * y_styles)?, (y * s_rgb | ToRGB output)
             x = None if drop_x else outs[0]
             if fold_rgb:
                 y_rgb = outs[-1]
@@ -520,8 +580,21 @@ class StylePlan:
         self._key, self._consts = key, (keep, structs, s_off, d_off)
         return self._consts
 
+    def _dcoef_multipliers(self, n, device, fp16_blocks):
+        """[n * d_tot] float32: over each demodulating layer's dcoefs, 2^e (SynthesisLayer.fp16_exponent) for the layers of
+        fp16_blocks, 1 for the others."""
+        sel = {m for b in fp16_blocks for m in b.modules()}
+        ex = lambda layer: layer.fp16_exponent() if layer in sel else 0
+        key = (n, str(device), tuple(ex(layer) for layer, _, demod, _ in self.entries if demod))
+        if getattr(self, '_mult_key', None) != key:
+            parts = [torch.full([n * layer.weight.shape[0]], 2.0 ** ex(layer), dtype=torch.float32)
+                     for layer, _, demod, _ in self.entries if demod]
+            self._mult_key, self._mult = key, torch.cat(parts).to(device)
+        return self._mult
+
     @torch.no_grad()
-    def run(self, ws):
+    def run(self, ws, fp16_blocks=()):
+        """fp16_blocks: blocks on fp16 operands (fp16_operands); their layers' dcoefs carry the 2^e of the fp16 weight copy."""
         import ctypes as C
         from .. import _lib as L
         ws = ws.detach().to(torch.float32).contiguous()
@@ -536,6 +609,8 @@ class StylePlan:
         with torch.cuda.device(ws.device):
             L.check(L.get_lib().ide3d_style_plan(L.ptr(ws), n, num_ws, w_dim, structs, len(self.entries), L.ptr(styles), L.ptr(dcoefs),
                                                  L.stream_ptr(ws.device)))
+        if len(fp16_blocks) and d_tot > 0:
+            dcoefs[:n * d_tot].mul_(self._dcoef_multipliers(n, ws.device, fp16_blocks))
         out = {}
         for k, (layer, _, demod, _) in enumerate(self.entries):
             i, o = structs[k].in_ch, structs[k].out_ch

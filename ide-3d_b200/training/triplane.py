@@ -217,12 +217,16 @@ class SynthesisNetwork(torch.nn.Module):
             idx += b.num_conv
         return voxel_ws, block_ws
 
-    def _style_plan(self, ws):
+    def _blocks(self):
+        return [getattr(self, f'vb{r}') for r in self.voxel_block_resolutions] + [getattr(self, f'b{r}') for r in self.block_resolutions]
+
+    def _style_plan(self, ws, fp16_blocks=()):
         """All styles / demodulation coefficients of the call in two launches (networks.StylePlan) when the blocks run the fp32
-        activation-scaled inference path on a CUDA device; None otherwise (every layer then computes its own, as the reference does)."""
+        activation-scaled inference path on a CUDA device; None otherwise (every layer then computes its own, as the reference does).
+        fp16_blocks: blocks that run on fp16 operands (networks.fp16_operands); their dcoefs carry each layer's 2^e."""
         if not (networks.STYLE_PLAN and ws.is_cuda) or (torch.is_grad_enabled() and (ws.requires_grad or any(p.requires_grad for p in self.parameters()))):
             return None
-        blocks = [getattr(self, f'vb{r}') for r in self.voxel_block_resolutions] + [getattr(self, f'b{r}') for r in self.block_resolutions]
+        blocks = self._blocks()
         if any(b.use_fp16 for b in blocks) or int(os.environ.get('IDE3D_FUSED_MODCONV_MIN_RES', networks.FUSED_MODCONV_MIN_RES)) <= max(b.resolution for b in blocks):
             return None
         plan = _STYLE_PLANS.get(self)                 # kept outside the module: the plan holds ctypes structs and is not picklable
@@ -232,7 +236,7 @@ class SynthesisNetwork(torch.nn.Module):
                 pairs.append((b, idx))
                 idx += b.num_conv
             plan = _STYLE_PLANS[self] = networks.StylePlan(pairs)
-        return plan.run(ws)
+        return plan.run(ws, fp16_blocks=fp16_blocks)
 
     def _chain_kwargs(self, blocks, block_kwargs):
         """Per-block keyword arguments that link consecutive blocks of one call (networks.FUSED_TORGB): every block but the last
@@ -282,9 +286,17 @@ class SynthesisNetwork(torch.nn.Module):
             raise ValueError(f'SynthesisNetwork: views must be >= 1, got {views}')
         voxel_ws, block_ws = self.split_ws(ws)
         block_kwargs = dict(noise_mode=noise_mode, force_fp32=force_fp32, fused_modconv=fused_modconv)
-        plan = self._style_plan(ws)
+        # fp16 convolution operands in the tri-plane backbone only: the super-resolution blocks write the image itself, and there one
+        # more rounding per convolution moves frames rendered at different batch sizes apart by 2 uint8 levels
+        # (tests/test_gpu_multiview.py allows 1)
+        backbone = [getattr(self, f'vb{r}') for r in self.voxel_block_resolutions]
+        fp16 = networks.fp16_operands(backbone, force_fp32=force_fp32, fused_modconv=fused_modconv)
+        plan = self._style_plan(ws, fp16_blocks=backbone if fp16 else ())
+        sr_kwargs = dict(block_kwargs)
         if plan is not None:
-            block_kwargs['style_plan'] = plan
+            block_kwargs['style_plan'] = sr_kwargs['style_plan'] = plan
+            if fp16:
+                block_kwargs['fp16_operands'] = True
         img_v, seg_v = self.backbone(voxel_ws, **block_kwargs)
         if views > 1:
             # the per-view part: SR styles are functions of the ws row alone, so the plan's rows are repeated rather than recomputed
@@ -292,7 +304,7 @@ class SynthesisNetwork(torch.nn.Module):
             if plan is not None:
                 rep = lambda t: None if t is None else t.repeat_interleave(views, 0)
                 sr_layers = {m for r in self.block_resolutions for m in getattr(self, f'b{r}').modules()}
-                block_kwargs['style_plan'] = {layer: (rep(st), rep(dc)) for layer, (st, dc) in plan.items() if layer in sr_layers}
+                sr_kwargs['style_plan'] = {layer: (rep(st), rep(dc)) for layer, (st, dc) in plan.items() if layer in sr_layers}
 
         kw = dict(self.rendering_kwargs)
         kw.update({k: v for k, v in (render_params or {}).items() if k in ('fov', 'num_steps', 'ray_start', 'ray_end',
@@ -319,7 +331,7 @@ class SynthesisNetwork(torch.nn.Module):
         # feat is [N, HW, 51]: already channels-last; keep that layout for the super-resolution blocks when they use it
         sr_fmt = torch.channels_last if networks.CHANNELS_LAST else torch.contiguous_format
         feat_img, seg_raw = maps[:, :N_FEAT].contiguous(memory_format=sr_fmt), maps[:, N_FEAT:]
-        img = self.superres(feat_img, block_ws, **block_kwargs)
+        img = self.superres(feat_img, block_ws, **sr_kwargs)
         out_size = (self.img_resolution, self.img_resolution)
         if return_dict:
             return dict(image=img, image_raw=feat_img[:, :self.img_channels],

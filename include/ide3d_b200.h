@@ -69,6 +69,10 @@ enum ide3d_status {
 };
 
 enum ide3d_dtype { IDE3D_F32 = 0, IDE3D_F16 = 1, IDE3D_F64 = 2 };
+/* Mixed-format code of the modulated-convolution epilogues and the skip add: IDE3D_DTYPE2(a, b) names two dtypes where
+ * those entry points take one.  Which tensors are `a` and which `b` is stated at each entry point; a plain ide3d_dtype
+ * keeps its meaning (every tensor of that dtype).  Accepted pairs are listed per entry point; others are IDE3D_UNSUPPORTED. */
+#define IDE3D_DTYPE2(a, b) ((a) | (((b) + 1) << 4))
 
 typedef void* ide3d_stream_t; /* cudaStream_t */
 
@@ -95,6 +99,8 @@ int ide3d_bias_act(const void* x, const void* b, const void* xref, const void* y
  * scale [n*c], noise [noise_batch * h*w] (noise_batch = 1 or n), b [c]: same dtype as x, each may be NULL.
  * Optional second output y2 = y * scale2[n,c] (scale2 [n*c]; y2 like y): the style modulation `x * styles` that opens
  * the NEXT modulated convolution (inversion/networks.py:100), written in the same pass; y may then be NULL.
+ * dtype IDE3D_DTYPE2(IDE3D_F32, IDE3D_F16) (channels_last only): x and every operand float32, y and y2 fp16 (each value
+ * computed in float32 and rounded once) -- the fp16 input of a convolution; act 1 (linear) or 3 (lrelu).
  * Forward only.  IDE3D_UNSUPPORTED when the vector width does not divide h*w (NCHW) or c (channels_last). */
 int ide3d_modconv_epilogue(const void* x, const void* scale, const void* noise, const void* b, void* y,
                            const void* scale2, void* y2, int dtype, int act, float alpha, float gain, float clamp,
@@ -109,7 +115,9 @@ int ide3d_modconv_epilogue(const void* x, const void* scale, const void* noise, 
  *         the block's ToRGB layer (modulated 1x1 convolution without demodulation, inversion/networks.py:700-707)
  * x, y, y2: [n, h*w, c]; scale, yscale, scale2, srgb [n*c]; wrgb [rgb_channels * c]; b [c]; brgb [rgb_channels] (may be NULL).
  * Each pixel's rgb sum runs in a fixed order without atomics (bit-identical reruns).  Forward only.
- * IDE3D_UNSUPPORTED unless dtype is IDE3D_F32, c % 4 == 0 and c <= 512. */
+ * dtype IDE3D_F32: every tensor float32.  IDE3D_DTYPE2(IDE3D_F16, IDE3D_F16): x, y and y2 fp16, every other operand and rgb
+ * float32; the arithmetic is float32 and each fp16 output is the float32 value rounded once.
+ * IDE3D_UNSUPPORTED for other dtypes, and unless c % 4 == 0 and c <= 512. */
 int ide3d_modconv_epilogue_rgb(const void* x, const void* scale, const void* noise, const void* b, const void* yscale,
                                void* y, const void* scale2, void* y2, const void* wrgb, const void* srgb, const void* brgb,
                                void* rgb, int64_t rgb_channels, int dtype, int act, float alpha, float gain, float clamp,
@@ -140,7 +148,8 @@ int ide3d_upfirdn2d(const ide3d_upfirdn2d_params* p, ide3d_stream_t stream);
  *     y = upfirdn2d(x, f, ...) + add + bias[c]
  * i.e. upsample2d of the running image (inversion/networks.py:841) fused with the `img.add_(y)` that follows (:844) and
  * with the ToRGB bias (:707).  add: same dtype, logical shape of y, element strides add_stride_{n,h,w}, channel stride 1
- * (it may be a channel slice of a wider channels_last tensor); bias [c] or NULL.  Only the channels_last patch kernel
+ * (it may be a channel slice of a wider channels_last tensor); bias [c] or NULL.  p->dtype IDE3D_DTYPE2(IDE3D_F32, IDE3D_F16):
+ * x, y and bias float32, add fp16 (the output of an fp16 convolution).  Only the channels_last patch kernel
  * implements it (x, y channels_last, C % 4 == 0, 4x4 filter, up/down in {1,2}); otherwise IDE3D_UNSUPPORTED. */
 int ide3d_upfirdn2d_add(const ide3d_upfirdn2d_params* p, const void* add, int64_t add_stride_n, int64_t add_stride_h,
                         int64_t add_stride_w, const void* bias, ide3d_stream_t stream);
@@ -152,6 +161,8 @@ int ide3d_upfirdn2d_add(const ide3d_upfirdn2d_params* p, const void* add, int64_
  *     y  = v                      (params->y; may be NULL when only y2 is wanted)
  *     y2 = v * scale2[n,c]        (optional: the next layer's style modulation, layout of y)
  * scale, b, scale2: dtype of x, [n*c] / [c] / [n*c]; noise: dtype of x, [noise_batch, out_h, out_w] dense; any may be NULL.
+ * p->dtype IDE3D_DTYPE2(IDE3D_F16, IDE3D_F16): x, y and y2 fp16; scale, noise, b, scale2, the filter and the arithmetic float32,
+ * each fp16 output rounded once from the float32 value.
  * Same kernel restrictions as ide3d_upfirdn2d_add (channels_last, C % 4 == 0, 4x4 filter); otherwise IDE3D_UNSUPPORTED. */
 typedef struct ide3d_fir_epilogue {
     const void *scale, *noise, *b, *scale2;
