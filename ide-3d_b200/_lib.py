@@ -167,6 +167,7 @@ class FeatL1Params(C.Structure):
 
 
 SEG_STEM_MAX_CLASSES = 31                              # IDE3D_SEG_STEM_MAX_CLASSES
+KNN_MAX_KTH = 16                                       # IDE3D_KNN_MAX_KTH
 
 
 class SegStemParams(C.Structure):
@@ -246,6 +247,10 @@ SIGNATURES = {
     'ide3d_seg_stem_bwd': (_i32, [_P(SegStemBwdParams), _vp]),
     'ide3d_seg_labels': (_i32, [_P(SegLabelsParams), _vp]),
     'ide3d_seg_labels_ac': (_i32, [_P(SegLabelsParams), _vp]),
+    'ide3d_knn_kth_dist_scratch_bytes': (_i64, [_i64, _i64, _i32]),
+    'ide3d_knn_kth_dist': (_i32, [_vp, _i64, _vp, _i64, _i32, _i32, _vp, _vp, _i64, _vp]),
+    'ide3d_knn_within_scratch_bytes': (_i64, [_i64, _i64]),
+    'ide3d_knn_within': (_i32, [_vp, _i64, _vp, _i64, _i32, _vp, _vp, _vp, _i64, _vp]),
 }
 
 

@@ -5,7 +5,8 @@
 After install(), `from training.volumetric_rendering import sample_camera_positions`, `from training.triplane
 import TriPlaneGenerator`, `from torch_utils.ops import upfirdn2d`, `import dnnlib` ... resolve to the sm_90a
 implementations, so gen_images.py / gen_videos.py / extract_shapes.py / viz/renderer.py run unchanged against a
-generator built by `random_init_generator()` (the reference checkpoints embed their own class source and are not
+generator built by `random_init_generator()`, and calc_metrics.py's subprocess_fn computes its metrics with
+`metrics.metric_main` (the reference checkpoints embed their own class source and are not
 available offline; see INTEGRATION.md).
 """
 
@@ -17,7 +18,9 @@ _ALIASES = [
     'torch_utils', 'torch_utils.custom_ops', 'torch_utils.misc', 'torch_utils.persistence', 'torch_utils.ops',
     'torch_utils.ops.bias_act', 'torch_utils.ops.upfirdn2d', 'torch_utils.ops.filtered_lrelu',
     'torch_utils.ops.conv2d_gradfix', 'torch_utils.ops.conv2d_resample', 'torch_utils.ops.fma',
-    'torch_utils.ops.grid_sample_gradfix',
+    'torch_utils.ops.grid_sample_gradfix', 'training.dataset', 'torch_utils.training_stats',
+    'metrics', 'metrics.metric_utils', 'metrics.frechet_inception_distance', 'metrics.kernel_inception_distance',
+    'metrics.precision_recall', 'metrics.inception_score', 'metrics.metric_main',
 ]
 
 

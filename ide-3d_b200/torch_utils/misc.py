@@ -65,3 +65,48 @@ class InfiniteSampler(torch.utils.data.Sampler):
 
     def __iter__(self):
         return itertools.islice(self._stream(), self.rank, None, self.num_replicas)
+
+
+def print_module_summary(module, inputs, max_nesting=3, skip_redundant=True):
+    """Run module(*inputs) once and print, for every submodule down to `max_nesting` levels, its parameter and buffer counts and its
+    first output's shape and dtype (torch_utils/misc.py:199); returns the outputs.  With skip_redundant, submodules that own no
+    parameter or buffer of their own and return a tensor already listed are left out."""
+    assert isinstance(module, torch.nn.Module) and not isinstance(module, torch.jit.ScriptModule)
+    assert isinstance(inputs, (tuple, list))
+    names = {m: n for n, m in module.named_modules()}
+    depth = {m: (0 if n == '' else n.count('.') + 1) for m, n in names.items()}
+    calls = []
+
+    def hook(mod, _inputs, outputs):
+        if depth[mod] <= max_nesting:
+            outs = outputs if isinstance(outputs, (tuple, list)) else [outputs]
+            calls.append((mod, [t for t in outs if isinstance(t, torch.Tensor)]))
+
+    hooks = [m.register_forward_hook(hook) for m in module.modules()]
+    try:
+        outputs = module(*inputs)
+    finally:
+        for h in hooks:
+            h.remove()
+
+    seen, rows, totals = set(), [], [0, 0]
+    for mod, outs in calls:
+        params = [t for t in mod.parameters() if id(t) not in seen]
+        bufs = [t for t in mod.buffers() if id(t) not in seen]
+        new_outs = [t for t in outs if id(t) not in seen]
+        seen |= {id(t) for t in params + bufs + new_outs}
+        if skip_redundant and not (params or bufs or new_outs):
+            continue
+        np_, nb = sum(t.numel() for t in params), sum(t.numel() for t in bufs)
+        totals[0] += np_
+        totals[1] += nb
+        name = '<top-level>' if mod is module else names[mod]
+        shape, dtype = (str(list(outs[0].shape)), str(outs[0].dtype).split('.')[-1]) if outs else ('-', '-')
+        rows.append([name, str(np_) if np_ else '-', str(nb) if nb else '-', shape, dtype])
+    table = [[type(module).__name__, 'Parameters', 'Buffers', 'Output shape', 'Datatype']] + rows + [['Total', str(totals[0]), str(totals[1]), '-', '-']]
+    widths = [max(len(r[i]) for r in table) for i in range(5)]
+    print()
+    for r in table:
+        print('  '.join(c.ljust(w) for c, w in zip(r, widths)))
+    print()
+    return outputs

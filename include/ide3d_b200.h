@@ -38,6 +38,8 @@
  *   ide3d_seg_stem_bwd        its gradients w.r.t. the three layers' weights (encoder fine-tuning)
  *   ide3d_seg_labels          the generator's class ids at image resolution (extension; the starting mask of an edit)
  *   ide3d_seg_labels_ac       dnnlib/seg_tools.py:101-117  argmax of BiSeNet's align_corners=True upsampling
+ *   ide3d_knn_kth_dist        metrics/precision_recall.py:17-52  k-th nearest-neighbour distance of every manifold row
+ *   ide3d_knn_within          metrics/precision_recall.py:53-60  does a probe fall inside some manifold point's radius
  *
  * Conventions
  *   - plain C: raw device pointers, sizes, strides (in ELEMENTS), a cudaStream_t passed as void*.
@@ -688,6 +690,27 @@ typedef struct ide3d_seg_labels_params {
 int ide3d_seg_labels(const ide3d_seg_labels_params* p, ide3d_stream_t stream);
 /* The same with align_corners=True (source position d * (in - 1) / (out - 1)): BiSeNet's upsampling (inversion/BiSeNet.py:249). */
 int ide3d_seg_labels_ac(const ide3d_seg_labels_params* p, ide3d_stream_t stream);
+
+/* k-nearest-neighbour distances of the precision / recall metric (metrics/precision_recall.py) over fp16 feature rows, D % 8 == 0,
+ * dense, 16-byte aligned.  One tensor-core GEMM main loop per call: squared distances |x|^2 + |y|^2 - 2 x.y (fp32 accumulation, norms
+ * in fp32 from the same fp16 values, negative values clamped to 0) are consumed in registers; the R x C matrix is never stored.
+ *   ide3d_knn_kth_dist: out[r] (fp32) = the kth smallest |rows[r] - cols[c]| over all c, 1 <= kth <= IDE3D_KNN_MAX_KTH, kth <= C.
+ *                       When rows is a slice of cols the row's own (zero) distance counts, as in the reference's
+ *                       kthvalue(nhood_size + 1).  scratch: ide3d_knn_kth_dist_scratch_bytes(R, C, kth) bytes, 256-byte aligned.
+ *   ide3d_knn_within:   flags[q] (uint8) = 1 if some j has |probes[q] - manifold[j]|^2 <= radius[j]^2 (radius fp32 [M]), else 0.
+ *                       A CTA stops once every probe it owns has a hit.  scratch: ide3d_knn_within_scratch_bytes(Q, M) bytes,
+ *                       256-byte aligned.
+ * IDE3D_INVALID for null pointers, kth outside [1, IDE3D_KNN_MAX_KTH] or above C, D % 8 != 0, misaligned pointers or too little
+ * scratch.  All but the last are decided from the arguments alone, before any CUDA call.  The kth_dist scratch size depends on the
+ * current device's SM count, so ide3d_knn_kth_dist_scratch_bytes and the scratch check of ide3d_knn_kth_dist query the device
+ * (cudaGetDevice, cudaDeviceGetAttribute); nothing is launched or read on the device before every check has passed. */
+#define IDE3D_KNN_MAX_KTH 16
+int64_t ide3d_knn_kth_dist_scratch_bytes(int64_t R, int64_t C, int kth);
+int ide3d_knn_kth_dist(const void* rows, int64_t R, const void* cols, int64_t C, int D, int kth, float* out, void* scratch,
+                       int64_t scratch_bytes, ide3d_stream_t stream);
+int64_t ide3d_knn_within_scratch_bytes(int64_t Q, int64_t M);
+int ide3d_knn_within(const void* probes, int64_t Q, const void* manifold, int64_t M, int D, const float* radius, uint8_t* flags,
+                     void* scratch, int64_t scratch_bytes, ide3d_stream_t stream);
 
 #ifdef __cplusplus
 }
