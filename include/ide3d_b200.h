@@ -40,6 +40,9 @@
  *   ide3d_seg_labels_ac       dnnlib/seg_tools.py:101-117  argmax of BiSeNet's align_corners=True upsampling
  *   ide3d_knn_kth_dist        metrics/precision_recall.py:17-52  k-th nearest-neighbour distance of every manifold row
  *   ide3d_knn_within          metrics/precision_recall.py:53-60  does a probe fall inside some manifold point's radius
+ *   ide3d_spectrum_accum      avg_spectra.py:161-166  average power spectrum `calc`: whitening, window, zero-padded fftn, |X|^2
+ *   ide3d_spectrum_finalize   avg_spectra.py:167  the division by the image count, in the reference's [P, P] bin order
+ *   ide3d_image_moments       avg_spectra.py:126-131  `stats`: sums of 1, x and x^2, as exact integers
  *
  * Conventions
  *   - plain C: raw device pointers, sizes, strides (in ELEMENTS), a cudaStream_t passed as void*.
@@ -711,6 +714,29 @@ int ide3d_knn_kth_dist(const void* rows, int64_t R, const void* cols, int64_t C,
 int64_t ide3d_knn_within_scratch_bytes(int64_t Q, int64_t M);
 int ide3d_knn_within(const void* probes, int64_t Q, const void* manifold, int64_t M, int D, const float* radius, uint8_t* flags,
                      void* scratch, int64_t scratch_bytes, ide3d_stream_t stream);
+
+/* Average power spectrum of avg_spectra.py `calc` (float64 throughout).  images uint8 [n, c, size, size] through strides in ELEMENTS
+ * (NCHW or NHWC); lut float64 [256] with lut[v] = (v - mean) / std (the caller's whitening, as the reference computes it); window
+ * float64 [size], the Kaiser window scaled by rsqrt(sum w^2).  P = size * interp.  For every image in index order
+ *     spectrum[k2, k1] += mean_c |sum_{n1, n2 < size} lut[x_c[n1, n2]] (window[n1] window[n2]) w_P^{n1 k1 + n2 k2}|^2
+ * over the half plane k2 <= P / 2: spectrum is the float64 accumulator [P / 2 + 1, P], k2-major, zeroed by the caller before the first
+ * call.  A pruned transform: rows, then columns, of the non-zero size x size block only; no P x P buffer.  Each bin has one owner
+ * that adds the images in order: no float atomics, reruns are bit-identical and any split of a sequence into calls gives the same bits.
+ * scratch: ide3d_spectrum_scratch_bytes(n, c, size, interp) bytes, 16-byte aligned.
+ * IDE3D_UNSUPPORTED unless size is a power of two in [16, 1024], interp is 1, 2, 4 or 8, P <= 4096 and 1 <= c <= 4 (the caller falls
+ * back to the reference's arithmetic); IDE3D_INVALID for null pointers or too little scratch.  Every check runs before any launch.
+ * ide3d_spectrum_finalize: out float64 [P, P] = the accumulator / count in the reference's (unshifted) bin order, the half plane
+ * k2 > P / 2 mirrored from out[k1, k2] = spectrum[P - k2, (P - k1) mod P]. */
+int64_t ide3d_spectrum_scratch_bytes(int n, int c, int size, int interp);
+int ide3d_spectrum_accum(const uint8_t* images, int n, int c, int size, int64_t stride_n, int64_t stride_c, int64_t stride_h,
+                         int64_t stride_w, const double* lut, const double* window, int interp, double* spectrum, void* scratch,
+                         int64_t scratch_bytes, ide3d_stream_t stream);
+int ide3d_spectrum_finalize(const double* spectrum, int size, int interp, int64_t count, double* out, ide3d_stream_t stream);
+
+/* avg_spectra.py `stats`: moments[0] += n * c * h * w, moments[1] += sum x, moments[2] += sum x^2 over uint8 images [n, c, h, w]
+ * (strides in ELEMENTS).  Exact integers at any dataset size; integer atomics, so the result does not depend on the order. */
+int ide3d_image_moments(const uint8_t* images, int n, int c, int h, int w, int64_t stride_n, int64_t stride_c, int64_t stride_h,
+                        int64_t stride_w, uint64_t* moments, ide3d_stream_t stream);
 
 #ifdef __cplusplus
 }
