@@ -255,6 +255,9 @@ SIGNATURES = {
     'ide3d_spectrum_accum': (_i32, [_vp, _i32, _i32, _i32, _i64, _i64, _i64, _i64, _vp, _vp, _i32, _vp, _vp, _i64, _vp]),
     'ide3d_spectrum_finalize': (_i32, [_vp, _i32, _i32, _i64, _vp, _vp]),
     'ide3d_image_moments': (_i32, [_vp, _i32, _i32, _i32, _i32, _i64, _i64, _i64, _i64, _vp, _vp]),
+    'ide3d_resample_u8_scratch_bytes': (_i64, [_i32, _i32, _i32, _i32, _i32, _i32, _i32]),
+    'ide3d_resample_u8': (_i32, [_vp, _i32, _i32, _i32, _i32, _i64, _i64, _i64, _vp, _i32, _i32, _i64, _i64, _i64, _i32, _vp, _vp, _i32,
+                                 _vp, _vp, _vp, _i64, _vp]),
 }
 
 

@@ -43,6 +43,7 @@
  *   ide3d_spectrum_accum      avg_spectra.py:161-166  average power spectrum `calc`: whitening, window, zero-padded fftn, |X|^2
  *   ide3d_spectrum_finalize   avg_spectra.py:167  the division by the image count, in the reference's [P, P] bin order
  *   ide3d_image_moments       avg_spectra.py:126-131  `stats`: sums of 1, x and x^2, as exact integers
+ *   ide3d_resample_u8         dataset_tool.py:226-256  PIL.Image.resize(LANCZOS) of 8-bit L / RGB images (Pillow's ImagingResample)
  *
  * Conventions
  *   - plain C: raw device pointers, sizes, strides (in ELEMENTS), a cudaStream_t passed as void*.
@@ -737,6 +738,25 @@ int ide3d_spectrum_finalize(const double* spectrum, int size, int interp, int64_
  * (strides in ELEMENTS).  Exact integers at any dataset size; integer atomics, so the result does not depend on the order. */
 int ide3d_image_moments(const uint8_t* images, int n, int c, int h, int w, int64_t stride_n, int64_t stride_c, int64_t stride_h,
                         int64_t stride_w, uint64_t* moments, ide3d_stream_t stream);
+
+/* Pillow's 8-bit two-pass resampler (libImaging/Resample.c, ImagingResample for L and RGB), table-driven and bit-identical.
+ * in uint8 [n, in_h, in_w, c] and out uint8 [n, out_h, out_w, c] through strides in BYTES (n, h, w; channels contiguous), so a centre
+ * crop is a pointer offset and a pitch and the output may be a window of a larger canvas.  c is 1 or 3.
+ * Tables, in HOST memory (the library checks them and copies them into scratch; they may be freed on return), one per axis:
+ *   bounds int32 [out, 2] = (first input index, tap count) and coeffs int32 [out, ksize], PIL's normalize_coeffs_8bpc weights
+ *   (22 fractional bits).  Every tap range must lie inside the input and have at most ksize taps.
+ * Passes as Pillow runs them: the horizontal pass (only if out_w != in_w) computes the rows bounds_y spans, first tap of the first
+ * output row to last tap of the last, into a uint8 intermediate; the vertical pass (only if out_h != in_h) reads it, or the input
+ * when the horizontal pass was skipped; with both skipped the call is a copy.  Each output value is
+ *     clamp((2^21 + sum_i v_i k_i) >> 22, 0, 255)                      in int32, as Pillow computes it.
+ * scratch: ide3d_resample_u8_scratch_bytes(n, c, in_h, out_h, out_w, ksize_x, ksize_y) bytes, 16-byte aligned.
+ * IDE3D_INVALID for null pointers, c not 1 or 3, non-positive sizes or ksizes, tables that do not fit the sizes or too little scratch,
+ * all decided before any CUDA call. */
+int64_t ide3d_resample_u8_scratch_bytes(int n, int c, int in_h, int out_h, int out_w, int ksize_x, int ksize_y);
+int ide3d_resample_u8(const uint8_t* in, int n, int c, int in_h, int in_w, int64_t in_stride_n, int64_t in_stride_h, int64_t in_stride_w,
+                      uint8_t* out, int out_h, int out_w, int64_t out_stride_n, int64_t out_stride_h, int64_t out_stride_w, int ksize_x,
+                      const int32_t* bounds_x, const int32_t* coeffs_x, int ksize_y, const int32_t* bounds_y, const int32_t* coeffs_y,
+                      void* scratch, int64_t scratch_bytes, ide3d_stream_t stream);
 
 #ifdef __cplusplus
 }
