@@ -258,6 +258,7 @@ SIGNATURES = {
     'ide3d_resample_u8_scratch_bytes': (_i64, [_i32, _i32, _i32, _i32, _i32, _i32, _i32]),
     'ide3d_resample_u8': (_i32, [_vp, _i32, _i32, _i32, _i32, _i64, _i64, _i64, _vp, _i32, _i32, _i64, _i64, _i64, _i32, _vp, _vp, _i32,
                                  _vp, _vp, _vp, _i64, _vp]),
+    'ide3d_style_grid': (_i32, [_vp, _i32, _i32, _i32, _i32, _i32, _i32, _i64, _i64, _i64, _i64, _vp, _i64, _i64, _vp]),
 }
 
 

@@ -156,6 +156,13 @@ def invalidate_caches(module):
 
 
 # ================================================================================================ synthesis
+def _gather(t, index):
+    """t[index] along dim 0 in one pass, keeping a channels_last layout (the fused skip passes and the chained convolutions expect it)."""
+    if t.dim() == 4 and t.is_contiguous(memory_format=torch.channels_last) and not t.is_contiguous():
+        return t.permute(0, 2, 3, 1).index_select(0, index).permute(0, 3, 1, 2)
+    return t.index_select(0, index)
+
+
 def upsample_seg(seg_raw, size):
     """Render-resolution semantic logits [N, 19, R, R] -> image resolution: bilinear, align_corners=False.  The rule of
     return_seg=True / return_dict; ide3d_video_frames (csrc/frames.cu) evaluates the same rule per pixel instead."""
@@ -256,10 +263,37 @@ class SynthesisNetwork(torch.nn.Module):
             out.append(kw)
         return out
 
-    def backbone(self, voxel_ws, **block_kwargs):
+    def prefix_blocks(self, rows):
+        """How many leading backbone blocks read none of the ws `rows` (their split_ws slices, torgb row included)."""
+        rows, idx = {int(r) for r in rows}, 0
+        for k, res in enumerate(self.voxel_block_resolutions):
+            b = getattr(self, f'vb{res}')
+            if rows.intersection(range(idx, idx + b.num_conv + b.num_torgb)):
+                return k
+            idx += b.num_conv
+        return len(self.voxel_block_resolutions)
+
+    def backbone(self, voxel_ws, shared_prefix=None, **block_kwargs):
         x = img_v = seg_v = None
         blocks = [getattr(self, f'vb{res}') for res in self.voxel_block_resolutions]
-        for block, cur_ws, kw in zip(blocks, voxel_ws, self._chain_kwargs(blocks, block_kwargs)):
+        kws = self._chain_kwargs(blocks, block_kwargs)
+        k = 0
+        if shared_prefix is not None:
+            # block k-1's torgb row is block k's conv0 row, so a prefix of un-mixed slices also fixes block k's conv0 styles within a
+            # group: the prefix runs the plain call's chained kwargs on the groups' first latents, x * styles included
+            k, first, inverse = shared_prefix
+            plan = block_kwargs.get('style_plan')
+            if plan is not None:
+                layers = {m for b in blocks[:k] for m in b.modules()}
+                plan = {layer: tuple(None if t is None else t.index_select(0, first) for t in sd)
+                        for layer, sd in plan.items() if layer in layers}
+            for block, cur_ws, kw in zip(blocks[:k], voxel_ws[:k], kws[:k]):
+                kw = dict(kw) if plan is None else dict(kw, style_plan=plan)
+                if kw.get('x_next_styles') is not None:
+                    kw['x_next_styles'] = kw['x_next_styles'].index_select(0, first)
+                x, img_v, seg_v = block(x, img_v, cur_ws.index_select(0, first), condition_img=seg_v, **kw)
+            x, img_v, seg_v = (None if t is None else _gather(t, inverse) for t in (x, img_v, seg_v))
+        for block, cur_ws, kw in zip(blocks[k:], voxel_ws[k:], kws[k:]):
             x, img_v, seg_v = block(x, img_v, cur_ws, condition_img=seg_v, **kw)
         return img_v, seg_v
 
@@ -276,15 +310,28 @@ class SynthesisNetwork(torch.nn.Module):
         return rgb
 
     def forward(self, ws, c=None, render_params=None, noise_mode='const', force_fp32=False, return_seg=False,
-                return_raw=False, return_dict=False, fused_modconv=None, views=1, **render_overrides):
+                return_raw=False, return_dict=False, fused_modconv=None, views=1, shared_prefix=None, **render_overrides):
         """views (extension): render every latent from `views` cameras with ONE backbone pass.  ws [N, num_ws, w_dim]; c [N * views, 25]
         in latent-major order (row i * views + j is view j of latent i); every output has N * views rows in that order.  The
         tri-plane backbone runs on the N latents, the renderer and the super-resolution blocks per view (their ws repeated per view).
-        seed= (a render override) may then hold N * views per-frame jitter seeds."""
+        seed= (a render override) may then hold N * views per-frame jitter seeds.
+        shared_prefix (extension) = (k, groups): groups holds N host ints, and latents with equal ids have equal ws rows for the first k
+        backbone blocks (prefix_blocks gives k for a set of differing rows).  Those k blocks then run once per group, on the group's first
+        latent, with the plain call's arithmetic, and their outputs are repeated per latent; the other blocks run per latent.  Only the
+        prefix blocks' batch changes, and with it possibly cuDNN's algorithm choice.  Nothing shared (k == 0 or all ids distinct) is
+        the plain call."""
         views = int(views)
         if views < 1:
             raise ValueError(f'SynthesisNetwork: views must be >= 1, got {views}')
         voxel_ws, block_ws = self.split_ws(ws)
+        if shared_prefix is not None:
+            k, groups = int(shared_prefix[0]), np.asarray(shared_prefix[1]).reshape(-1)
+            if not 0 <= k <= len(self.voxel_block_resolutions) or groups.shape[0] != ws.shape[0]:
+                raise ValueError(f'SynthesisNetwork: shared_prefix needs 0 <= k <= {len(self.voxel_block_resolutions)} and {ws.shape[0]} '
+                                 f'group ids, got k={k} and {groups.shape[0]}')
+            _, first, inverse = np.unique(groups, return_index=True, return_inverse=True)
+            shared_prefix = None if k == 0 or len(first) == len(groups) else \
+                (k, torch.from_numpy(first).to(ws.device), torch.from_numpy(inverse.reshape(-1)).to(ws.device))
         block_kwargs = dict(noise_mode=noise_mode, force_fp32=force_fp32, fused_modconv=fused_modconv)
         # fp16 convolution operands in the tri-plane backbone only: the super-resolution blocks write the image itself, and there one
         # more rounding per convolution moves frames rendered at different batch sizes apart by 2 uint8 levels
@@ -297,7 +344,7 @@ class SynthesisNetwork(torch.nn.Module):
             block_kwargs['style_plan'] = sr_kwargs['style_plan'] = plan
             if fp16:
                 block_kwargs['fp16_operands'] = True
-        img_v, seg_v = self.backbone(voxel_ws, **block_kwargs)
+        img_v, seg_v = self.backbone(voxel_ws, shared_prefix=shared_prefix, **block_kwargs)
         if views > 1:
             # the per-view part: SR styles are functions of the ws row alone, so the plan's rows are repeated rather than recomputed
             block_ws = [w.repeat_interleave(views, 0) for w in block_ws]

@@ -44,6 +44,7 @@
  *   ide3d_spectrum_finalize   avg_spectra.py:167  the division by the image count, in the reference's [P, P] bin order
  *   ide3d_image_moments       avg_spectra.py:126-131  `stats`: sums of 1, x and x^2, as exact integers
  *   ide3d_resample_u8         dataset_tool.py:226-256  PIL.Image.resize(LANCZOS) of 8-bit L / RGB images (Pillow's ImagingResample)
+ *   ide3d_style_grid          apps/style_mixing.py:100-153  the uint8 conversion and the canvas paste loop of the style-mixing grid
  *
  * Conventions
  *   - plain C: raw device pointers, sizes, strides (in ELEMENTS), a cudaStream_t passed as void*.
@@ -757,6 +758,19 @@ int ide3d_resample_u8(const uint8_t* in, int n, int c, int in_h, int in_w, int64
                       uint8_t* out, int out_h, int out_w, int64_t out_stride_n, int64_t out_stride_h, int64_t out_stride_w, int ksize_x,
                       const int32_t* bounds_x, const int32_t* coeffs_x, int ksize_y, const int32_t* bounds_y, const int32_t* coeffs_y,
                       void* scratch, int64_t scratch_bytes, ide3d_stream_t stream);
+
+/* The style-mixing grid of style_mixing.py:139-153 as uint8 HWC canvases: grid rows first_row .. first_row + rows - 1 of a grid of
+ * cols + 1 columns, each grid row height pixels tall, every canvas (cols + 1) * width pixels wide.  Slot (g, j) holds cell
+ * g * (cols + 1) + j - 1 (canvas order: the column seeds, then per row seed its un-mixed image followed by its mixed cells); slot (0, 0)
+ * is black.  cells fp32 [ncells * views, 3, height, width], element strides, cell-major (row k * views + v is view v of the call's k-th
+ * cell); the call reads the cells of its rows only, the first being that of slot (first_row, 0), or (0, 1) for first_row 0.
+ * Each byte is (x * 127.5 + 128).clamp(0, 255).to(uint8) as torch computes it on the device (style_mixing.py:101).
+ * out: byte (gi, v, y, x, c) of local grid row gi at out + gi * out_stride_row + v * out_stride_view + (y * (cols + 1) * width + x) * 3
+ * + c.  One launch for every view.  IDE3D_INVALID for bad sizes, a canvas wider than 2^30 bytes or taller than 262140 pixels, or null
+ * pointers, decided before any CUDA call; rows == 0 is a no-op. */
+int ide3d_style_grid(const float* cells, int first_row, int rows, int cols, int views, int height, int width, int64_t stride_n,
+                     int64_t stride_c, int64_t stride_h, int64_t stride_w, uint8_t* out, int64_t out_stride_row, int64_t out_stride_view,
+                     ide3d_stream_t stream);
 
 #ifdef __cplusplus
 }
