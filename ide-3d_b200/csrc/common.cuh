@@ -69,10 +69,11 @@ template <typename T>
 __host__ __device__ inline T ceil_div(T a, T b) { return (a + b - 1) / b; }
 
 // Grid of a persistent kernel: as many CTAs of `threads` threads and `smem` bytes of dynamic shared memory as are resident on
-// the device at once, at most `max_ctas` (the CTAs that have work).  Raises the kernel's dynamic shared-memory limit to `smem`.
+// the device at once, at most `max_ctas` (the CTAs that have work).  Raises the kernel's dynamic shared-memory limit to `smem`
+// when `smem` exceeds the 48 KB every kernel may use without it.
 template <typename Kernel>
 inline int persistent_grid(Kernel kern, int threads, size_t smem, long long max_ctas, int& grid) {
-    IDE3D_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (smem > 48 * 1024) IDE3D_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int per_sm = 1;
     IDE3D_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
     if (per_sm < 1) per_sm = 1;

@@ -155,6 +155,7 @@ extern "C" int ide3d_filtered_lrelu(const ide3d_filtered_lrelu_params* q, ide3d_
     IDE3D_REQUIRE(q && q->x && q->y && q->fu && q->fd, "filtered_lrelu: null tensor");
     IDE3D_REQUIRE(q->dtype == IDE3D_F32 || q->dtype == IDE3D_F16, "x and b must be float16 or float32");
     IDE3D_REQUIRE(q->up >= 1 && q->down >= 1, "up and down must be at least 1");
+    IDE3D_REQUIRE(q->x_c > 0 && q->x_n > 0 && q->y_w > 0 && q->y_h > 0, "filtered_lrelu: y is empty");
     IDE3D_REQUIRE(!(q->write_signs && q->read_signs), "filtered_lrelu: cannot read and write signs at once");
     // separable filters only (fu_h == 0), or 1x1 "full" filters when the factor is 1 (filtered_lrelu.py:178-181)
     const bool fu_ok = (q->fu_h == 0) || (q->fu_h == 1 && q->fu_w == 1);

@@ -8,7 +8,7 @@
 // one shared-memory load and one store per UP*TU + FD fused multiply-adds (0.08 accesses / FMA; the round-1 kernel spent
 // 0.5 / FMA on shared-memory windows and was shared-memory bound at 5 % of the HBM roofline).
 //
-//   s_in [IH][BW][CB]   input tile in the tensor's own dtype, staged by ONE TMA box load per tile (cp.async.bulk.tensor, 3-D map
+//   s_in [IH][BW][CB]   input tile in the tensor's own dtype, staged by ONE TMA box load per tile (tma_load_3d / _4d, 3-D map
 //                       W x H x planes for NCHW, 4-D map C x W x H x N for channels-last); out-of-image texels arrive as zeros
 //                       (the TMA unit's out-of-bounds fill = the op's zero padding).  The load of tile i+1 is issued as soon as
 //                       pass A of tile i has consumed the buffer and overlaps passes B and C.  Tensors the TMA unit cannot
@@ -26,9 +26,8 @@
 // e_start = UP * b0 - UP + 1 (b0 = ceil(e_first / UP)) and produces e_start + n for n = 0, 1, 2, ...; D = e_first - e_start is the
 // number of leading samples to skip (< UP).  Loops run over blocks of P input samples, P chosen so that every ring slot, filter
 // phase, down-sampling phase and sign-nibble position is a compile-time constant inside the unrolled block body.
-#include <cuda.h>
-
 #include "common.cuh"
+#include "tma.cuh"
 
 namespace ide3d {
 
@@ -105,29 +104,6 @@ struct Geom {
     static_assert((UP * P) % FD == 0 && (UP * P) % DOWN == 0 && (UP * P) % 4 == 0 && P % TU == 0 && FD % DOWN == 0, "march block");
     static_assert(CB == 1 || ((TOW * DOWN / UP) >= 1), "tile");
 };
-
-__device__ __forceinline__ unsigned smem_addr(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void bar_init(unsigned long long* bar) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_addr(bar)) : "memory");
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void bar_wait(unsigned long long* bar, unsigned parity) {
-    unsigned ok = 0;
-    while (!ok) {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
-                     : "=r"(ok) : "r"(smem_addr(bar)), "r"(parity) : "memory");
-    }
-}
-__device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, unsigned long long* bar, int x, int y, int z, unsigned bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_addr(bar)), "r"(bytes) : "memory");
-    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-                 ::"r"(smem_addr(dst)), "l"(map), "r"(smem_addr(bar)), "r"(x), "r"(y), "r"(z) : "memory");
-}
-__device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, unsigned long long* bar, int c, int x, int y, int n, unsigned bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_addr(bar)), "r"(bytes) : "memory");
-    asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-                 ::"r"(smem_addr(dst)), "l"(map), "r"(smem_addr(bar)), "r"(c), "r"(x), "r"(y), "r"(n) : "memory");
-}
 
 // -------------------------------------------------------------------------------------------------------------------------
 // pass B of one item: intermediate row `row` (g1, element stride CB), x segment starting at output column o0.
@@ -232,7 +208,7 @@ filtered_lrelu_fused2_kernel(const FlFusedArgs p, int tiles_x, int tiles_y, int 
     float* g1 = reinterpret_cast<float*>(base + G::kInBytes);
     float* w = g1 + G::kG1Floats + G::kG1Slack;
     float* taps = w + G::kWFloats + G::kWSlack;            // [4][32]: up (vertical), up (horizontal, * gains), down (horizontal), down (vertical)
-    unsigned long long* bar = reinterpret_cast<unsigned long long*>(g1 + ((G::kG1Floats + G::kG1Slack + G::kWFloats + G::kWSlack + 4 * 32 + 3) / 4) * 4);    // 16-byte aligned: g1 starts on a 128-byte boundary
+    uint64_t* bar = reinterpret_cast<uint64_t*>(g1 + ((G::kG1Floats + G::kG1Slack + G::kWFloats + G::kWSlack + 4 * 32 + 3) / 4) * 4);    // 16-byte aligned: g1 starts on a 128-byte boundary
     const int tid = threadIdx.x;
 
     const float act_gain = p.gain * (float)(UP * UP) * (p.one_u ? 1.f / p.fu[0] : 1.f);
@@ -273,11 +249,19 @@ filtered_lrelu_fused2_kernel(const FlFusedArgs p, int tiles_x, int tiles_y, int 
         int n, cb, tx, ty;
         decode(blk, n, cb, tx, ty);
         const int ix_t = tx * (G::TOW * DOWN / UP) + ix0, iy_t = ty * (G::TOH * DOWN / UP) + iy0;
-        if (CB == 1) tma_load_3d(s_in, &tmap, bar, ix_t - shift_x, iy_t, n * p.xc + cb, kBoxBytes);
-        else tma_load_4d(s_in, &tmap, bar, cb * CB, ix_t, iy_t, n, kBoxBytes);
+        if (CB == 1) {
+            const int x = ix_t - shift_x, plane = n * p.xc + cb;
+            mbar_arrive_expect_tx(bar, kBoxBytes);
+            tma_load_3d(s_in, &tmap, bar, x, iy_t, plane);
+        } else {
+            const int c = cb * CB;
+            mbar_arrive_expect_tx(bar, kBoxBytes);
+            tma_load_4d(s_in, &tmap, bar, c, ix_t, iy_t, n);
+        }
     };
     if (tid == 0) {
-        bar_init(bar);
+        mbar_init(bar, 1);
+        mbar_fence_init();
         if (use_tma && (long long)blockIdx.x < total) issue(blockIdx.x);
     }
     __syncthreads();
@@ -293,7 +277,7 @@ filtered_lrelu_fused2_kernel(const FlFusedArgs p, int tiles_x, int tiles_y, int 
         const int bx0 = ix_t - shift_x;                                       // global column of box column 0
 
         if (use_tma) {
-            bar_wait(bar, it & 1);
+            mbar_wait(bar, it & 1);
         } else {
             // staged by the threads: same [row][col][c] layout, zeros outside the image / beyond the channel count
             const T* xin = (const T*)p.x + (long long)n * p.sxn;
@@ -431,19 +415,6 @@ filtered_lrelu_fused2_kernel(const FlFusedArgs p, int tiles_x, int tiles_y, int 
 }
 
 // ---- host side --------------------------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn encode_tiled() {
-    static EncodeTiledFn fn = []() -> EncodeTiledFn {
-        void* ptr = nullptr;
-        cudaDriverEntryPointQueryResult qr;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qr) != cudaSuccess || qr != cudaDriverEntryPointSuccess) return nullptr;
-        return (EncodeTiledFn)ptr;
-    }();
-    return fn;
-}
-
 template <typename T, int UP, int DOWN, int FU, int FD, int CB>
 static bool make_map(const FlFusedArgs& a, CUtensorMap& map) {
     using G = Geom<T, UP, DOWN, FU, FD, CB>;
@@ -486,16 +457,11 @@ static int launch_mode(const FlFusedArgs& a, cudaStream_t st) {
     const int shift = (CB == 1) ? pmod(ix0, G::kVec) : 0;
     auto kern = filtered_lrelu_fused2_kernel<T, UP, DOWN, FU, FD, CB, MODE, FAST>;
     const int smem = G::kSmem;
-    IDE3D_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     const int tiles_x = ceil_div(a.yw, G::TOW), tiles_y = ceil_div(a.yh, G::TOH);
     const int cblocks = ceil_div(a.xc, CB);
-    const long long total = (long long)tiles_x * tiles_y * cblocks * a.xn;
-    int per_sm = 1;
-    IDE3D_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, G::kThreads, smem));
-    if (per_sm < 1) per_sm = 1;
-    long long grid = (long long)sm_count() * per_sm;
-    if (grid > total) grid = total;
-    kern<<<(unsigned)grid, G::kThreads, smem, st>>>(a, tiles_x, tiles_y, cblocks, tma ? 1 : 0, shift, map);
+    int grid = 0, rc;
+    if ((rc = persistent_grid(kern, G::kThreads, smem, (long long)tiles_x * tiles_y * cblocks * a.xn, grid)) != IDE3D_OK) return rc;
+    kern<<<grid, G::kThreads, smem, st>>>(a, tiles_x, tiles_y, cblocks, tma ? 1 : 0, shift, map);
     IDE3D_CHECK_LAUNCH("filtered_lrelu_fused2_kernel");
     return IDE3D_OK;
 }

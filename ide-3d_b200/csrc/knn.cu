@@ -2,7 +2,7 @@
 // ide3d_knn_within.  Both are one Hopper GEMM main loop over fp16 features with the distance epilogue in registers:
 //
 //   CTA = 128 rows (two consumer warpgroups of 64) x all column tiles of its split (128 columns each).  A producer warp streams
-//   the row tile's and the column tile's 64-wide K slices with cp.async.bulk.tensor (128-byte swizzle) into a 4-stage
+//   the row tile's and the column tile's 64-wide K slices with tma_load_2d (128-byte swizzle) into a 4-stage
 //   full / empty mbarrier ring; each consumer warpgroup runs wgmma m64n128k16 (fp16 operands, fp32 accumulators) over the ring
 //   and turns its 64 x 128 dot products into squared distances max(|x|^2 + |y|^2 - 2 x.y, 0) with fp32 row norms of the same
 //   fp16 values (knn_norms_kernel).  The R x C matrix is never stored.
@@ -17,10 +17,9 @@
 // Column tiles are walked in ascending order by every CTA, so the CTAs resident at the same time stream the same column tiles
 // through L2.  Splitting the columns over several CTAs (when the row tiles alone do not fill the device) keeps that order inside
 // each split.
-#include <cuda.h>
-
 #include "common.cuh"
 #include "tc_ptx.cuh"
+#include "tma.cuh"
 
 namespace ide3d {
 namespace {
@@ -42,24 +41,6 @@ struct KnnArgs {
     uint8_t* flags;          // within
     float* partial;          // kth_dist: [splits, R, K]
 };
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, unsigned count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(tc::smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(tc::smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, unsigned parity) {
-    unsigned ok = 0;
-    while (!ok) {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
-                     : "=r"(ok) : "r"(tc::smem_u32(bar)), "r"(parity) : "memory");
-    }
-}
-__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, uint64_t* bar, int k, int row) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                 ::"r"(tc::smem_u32(dst)), "l"(map), "r"(tc::smem_u32(bar)), "r"(k), "r"(row) : "memory");
-}
 
 // sorted insertion into the K smallest seen so far (t ascending)
 template <int K>
@@ -118,7 +99,7 @@ __global__ void __launch_bounds__(kThreads, 1) knn_tile_kernel(const __grid_cons
         }
         mbar_init(&tile_done[0], 1);
         mbar_init(&tile_done[1], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_fence_init();
     }
     __syncthreads();
 
@@ -133,7 +114,7 @@ __global__ void __launch_bounds__(kThreads, 1) knn_tile_kernel(const __grid_cons
                 for (int kc = 0; kc < a.kchunks; ++kc, ++it) {
                     const int s = it % kStages;
                     if (it >= kStages) mbar_wait(&empty[s], (it / kStages - 1) & 1);
-                    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(tc::smem_u32(&full[s])), "r"(kStageBytes) : "memory");
+                    mbar_arrive_expect_tx(&full[s], kStageBytes);
                     unsigned char* st = base + s * kStageBytes;
                     tma_load_2d(st, &rows_map, &full[s], kc * kBK, row0);
                     tma_load_2d(st + kTileBytes, &cols_map, &full[s], kc * kBK, ct * kBN);
@@ -158,8 +139,8 @@ __global__ void __launch_bounds__(kThreads, 1) knn_tile_kernel(const __grid_cons
         for (int kc = 0; kc < a.kchunks; ++kc, ++it) {
             const int s = it % kStages;
             mbar_wait(&full[s], (it / kStages) & 1);
-            const uint32_t a_addr = tc::smem_u32(base + s * kStageBytes) + wg * 64 * 128;
-            const uint32_t b_addr = tc::smem_u32(base + s * kStageBytes + kTileBytes);
+            const uint32_t a_addr = smem_u32(base + s * kStageBytes) + wg * 64 * 128;
+            const uint32_t b_addr = smem_u32(base + s * kStageBytes + kTileBytes);
             tc::wgmma_fence();
 #pragma unroll
             for (int kk = 0; kk < kBK / 16; ++kk)
@@ -279,22 +260,9 @@ __global__ void __launch_bounds__(256) knn_kth_merge_kernel(const float* __restr
     out[r] = sqrtf(v);
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn encode_tiled() {
-    static EncodeTiledFn fn = []() -> EncodeTiledFn {
-        void* ptr = nullptr;
-        cudaDriverEntryPointQueryResult qr;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qr) != cudaSuccess || qr != cudaDriverEntryPointSuccess) return nullptr;
-        return (EncodeTiledFn)ptr;
-    }();
-    return fn;
-}
-
 // [n, D] fp16 row-major, 128 x 64 boxes with the 128-byte swizzle; rows past n and K past D read as zero
 int make_map(CUtensorMap* map, const void* x, int64_t n, int D) {
-    if (encode_tiled() == nullptr) IDE3D_FAIL(IDE3D_UNSUPPORTED, "knn: cuTensorMapEncodeTiled is not available");
+    if (encode_tiled() == nullptr) IDE3D_FAIL(IDE3D_UNSUPPORTED, "knn: the driver provides no tensor-map encoder");
     const cuuint64_t dims[2] = {(cuuint64_t)D, (cuuint64_t)n};
     const cuuint64_t strides[1] = {(cuuint64_t)D * 2};
     const cuuint32_t box[2] = {(cuuint32_t)kBK, (cuuint32_t)kBM};
@@ -302,7 +270,7 @@ int make_map(CUtensorMap* map, const void* x, int64_t n, int D) {
     const CUresult r = encode_tiled()(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(x), dims, strides, box, estr,
                                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) IDE3D_FAIL(IDE3D_UNSUPPORTED, "knn: cuTensorMapEncodeTiled failed (%d)", (int)r);
+    if (r != CUDA_SUCCESS) IDE3D_FAIL(IDE3D_UNSUPPORTED, "knn: encoding the tensor map failed (%d)", (int)r);
     return IDE3D_OK;
 }
 

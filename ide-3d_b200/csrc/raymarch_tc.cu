@@ -110,8 +110,8 @@ __global__ void __launch_bounds__(kTcThreads) raymarch_tc_kernel(const TcArgs a)
     const int W = a.tex.w, H = a.tex.h;
     unsigned char* a_hi = tile_base + wg * kStageBytes;
     unsigned char* a_lo = a_hi + kTileBytes;
-    const uint64_t ah0 = tc::make_sdesc_sw128(tc::smem_u32(a_hi)), al0 = tc::make_sdesc_sw128(tc::smem_u32(a_lo));
-    const uint64_t wh0 = tc::make_sdesc_sw128(tc::smem_u32(w_hi)), wl0 = tc::make_sdesc_sw128(tc::smem_u32(w_lo));
+    const uint64_t ah0 = tc::make_sdesc_sw128(smem_u32(a_hi)), al0 = tc::make_sdesc_sw128(smem_u32(a_lo));
+    const uint64_t wh0 = tc::make_sdesc_sw128(smem_u32(w_hi)), wl0 = tc::make_sdesc_sw128(smem_u32(w_lo));
     const int unit_stride = kWarpgroups * gridDim.x;
 
     for (int unit = blockIdx.x * kWarpgroups + wg; unit < a.num_units; unit += unit_stride) {

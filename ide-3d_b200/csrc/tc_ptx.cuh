@@ -7,10 +7,10 @@
 #include <cuda_bf16.h>
 #include <stdint.h>
 
+#include "tma.cuh"
+
 namespace ide3d {
 namespace tc {
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 // ---------------------------------------------------------------------------------------- fences / barriers
 // generic-proxy shared-memory writes -> visible to the async proxy (wgmma operand reads)

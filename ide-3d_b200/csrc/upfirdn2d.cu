@@ -13,12 +13,12 @@
 //     padding (pad mod up) is a template parameter, so every tap -> window index is a constant and there
 //     are no divisions, no bounds checks and no wasted zero taps in the inner loop.
 //   * generic kernel: any strides (channels_last included), any filter, one thread per output.
-#include <cuda.h>
 #include <stdlib.h>
 
 #include <type_traits>
 
 #include "common.cuh"
+#include "tma.cuh"
 
 namespace ide3d {
 
@@ -214,26 +214,9 @@ __global__ void __launch_bounds__(256) upfirdn2d_patch_kernel(const UpfirArgs p,
 
 // ------------------------------------------------------------------------------------------
 // TMA-staged flavour of the patch kernel (fp32 / fp16, dense NCHW): the input tile is fetched by ONE
-// cp.async.bulk.tensor (3-D map: W x H x planes, box = tile), out-of-image elements are zero-filled by the TMA unit
+// tma_load_3d (3-D map: W x H x planes, box = tile), out-of-image elements are zero-filled by the TMA unit
 // (negative / overflowing coordinates included), two tiles are in flight per block (double buffer + mbarrier) so the
 // load of tile i+1 overlaps the FIR of tile i, and no thread spends instructions on staging.
-__device__ __forceinline__ unsigned smem_addr(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void tma_bar_init(unsigned long long* bar) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_addr(bar)) : "memory");
-}
-__device__ __forceinline__ void tma_load_tile(void* dst, const CUtensorMap* map, unsigned long long* bar, int x, int y, int z, unsigned bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_addr(bar)), "r"(bytes) : "memory");
-    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-                 ::"r"(smem_addr(dst)), "l"(map), "r"(smem_addr(bar)), "r"(x), "r"(y), "r"(z) : "memory");
-}
-__device__ __forceinline__ void tma_bar_wait(unsigned long long* bar, unsigned parity) {
-    unsigned ok = 0;
-    while (!ok) {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
-                     : "=r"(ok) : "r"(smem_addr(bar)), "r"(parity) : "memory");
-    }
-}
-
 template <typename T, int UX, int UY, int DX, int DY, int FW, int FH, int PHX, int PHY>
 struct TmaGeom {
     using AX = Axis<UX, DX, FW, PHX>;
@@ -258,7 +241,7 @@ __global__ void __launch_bounds__(256) upfirdn2d_patch_tma_kernel(const UpfirArg
     extern __shared__ unsigned char tma_raw[];
     unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(tma_raw) + 127) & ~(uintptr_t)127);
     T* tiles[2] = {reinterpret_cast<T*>(base), reinterpret_cast<T*>(base + GM::kTileBytes)};
-    unsigned long long* bars = reinterpret_cast<unsigned long long*>(base + 2 * GM::kTileBytes);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(base + 2 * GM::kTileBytes);
 
     float fk[FH][FW];
 #pragma unroll
@@ -284,11 +267,14 @@ __global__ void __launch_bounds__(256) upfirdn2d_patch_tma_kernel(const UpfirArg
     auto issue = [&](long long blk, int buf) {
         int pl, ox_t, oy_t;
         coords(blk, pl, ox_t, oy_t);
-        tma_load_tile(tiles[buf], &tmap, &bars[buf], ox_t * DX / UX - ax + AX::lo() - shift, oy_t * DY / UY - ay + AY::lo(), pl, kBytes);
+        T* dst = tiles[buf];
+        const int x = ox_t * DX / UX - ax + AX::lo() - shift, y = oy_t * DY / UY - ay + AY::lo();
+        mbar_arrive_expect_tx(&bars[buf], kBytes);
+        tma_load_3d(dst, &tmap, &bars[buf], x, y, pl);
     };
     if (threadIdx.x == 0) {
-        tma_bar_init(&bars[0]); tma_bar_init(&bars[1]);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_init(&bars[0], 1); mbar_init(&bars[1], 1);
+        mbar_fence_init();
         if ((long long)blockIdx.x < total) issue(blockIdx.x, 0);
     }
     __syncthreads();
@@ -301,7 +287,7 @@ __global__ void __launch_bounds__(256) upfirdn2d_patch_tma_kernel(const UpfirArg
         int plane, ox_t, oy_t;
         coords(blk, plane, ox_t, oy_t);
         const int n = plane / p.in_c, c = plane - n * p.in_c;
-        tma_bar_wait(&bars[cur], (it >> 1) & 1);
+        mbar_wait(&bars[cur], (it >> 1) & 1);
         if constexpr (sizeof(T) == 4) {
             patch_compute_store<T, UX, UY, DX, DY, FW, FH, PHX, PHY, GM::BW>(p, reinterpret_cast<const float*>(tiles[cur]) + shift, fk, n, c, ox_t, oy_t);
         } else {
@@ -345,19 +331,6 @@ __global__ void __launch_bounds__(256) upfirdn2d_generic_kernel(const UpfirArgs 
 }
 
 // ---- host side of the TMA path -----------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn encode_tiled() {
-    static EncodeTiledFn fn = []() -> EncodeTiledFn {
-        void* ptr = nullptr;
-        cudaDriverEntryPointQueryResult qr;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qr) != cudaSuccess || qr != cudaDriverEntryPointSuccess) return nullptr;
-        return (EncodeTiledFn)ptr;
-    }();
-    return fn;
-}
-
 // can the TMA unit describe this input?  dense NCHW (planes equally spaced), 16-byte aligned base and row pitch
 template <typename T>
 static bool tma_eligible(const UpfirArgs& p) {
@@ -380,18 +353,13 @@ static int launch_patch_tma(const UpfirArgs& p, cudaStream_t st_) {
     const CUresult r = encode_tiled()(&map, sizeof(T) == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3,
                                       const_cast<void*>(p.x), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                       CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) IDE3D_FAIL(IDE3D_UNSUPPORTED, "upfirdn2d: cuTensorMapEncodeTiled failed (%d)", (int)r);
+    if (r != CUDA_SUCCESS) IDE3D_FAIL(IDE3D_UNSUPPORTED, "upfirdn2d: encoding the tensor map failed (%d)", (int)r);
     auto kern = upfirdn2d_patch_tma_kernel<T, UX, UY, DX, DY, FW, FH, PHX, PHY>;
     const size_t smem = GM::kSmem;
-    if (smem > 48 * 1024) IDE3D_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int tiles_x = ceil_div(p.out_w, kTile), tiles_y = ceil_div(p.out_h, kTile);
-    const long long total = (long long)tiles_x * tiles_y * p.in_c * p.in_n;
-    int per_sm = 1;
-    IDE3D_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, smem));
-    if (per_sm < 1) per_sm = 1;
-    long long grid = (long long)sm_count() * per_sm;
-    if (grid > total) grid = total;
-    kern<<<(unsigned)grid, 256, smem, st_>>>(p, tiles_x, tiles_y, map);
+    int grid = 0, rc;
+    if ((rc = persistent_grid(kern, 256, smem, (long long)tiles_x * tiles_y * p.in_c * p.in_n, grid)) != IDE3D_OK) return rc;
+    kern<<<grid, 256, smem, st_>>>(p, tiles_x, tiles_y, map);
     IDE3D_CHECK_LAUNCH("upfirdn2d_patch_tma_kernel");
     return IDE3D_OK;
 }
@@ -418,15 +386,10 @@ static int launch_patch(const UpfirArgs& p, cudaStream_t st_) {
     const size_t smem = (size_t)pitch * AY::kTileIn * sizeof(S) + 16;
     void (*kern)(const UpfirArgs, int, int) = upfirdn2d_patch_kernel<T, UX, UY, DX, DY, FW, FH, PHX, PHY, false>;
     if constexpr (sizeof(T) == 4) { if (vec) kern = upfirdn2d_patch_kernel<T, UX, UY, DX, DY, FW, FH, PHX, PHY, true>; }
-    if (smem > 48 * 1024) IDE3D_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int tiles_x = ceil_div(p.out_w, kTile), tiles_y = ceil_div(p.out_h, kTile);
-    const long long total = (long long)tiles_x * tiles_y * p.in_c * p.in_n;
-    int per_sm = 1;
-    IDE3D_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, smem));
-    if (per_sm < 1) per_sm = 1;
-    long long grid = (long long)sm_count() * per_sm;
-    if (grid > total) grid = total;
-    kern<<<(unsigned)grid, 256, smem, st_>>>(p, tiles_x, tiles_y);
+    int grid = 0, rc;
+    if ((rc = persistent_grid(kern, 256, smem, (long long)tiles_x * tiles_y * p.in_c * p.in_n, grid)) != IDE3D_OK) return rc;
+    kern<<<grid, 256, smem, st_>>>(p, tiles_x, tiles_y);
     IDE3D_CHECK_LAUNCH("upfirdn2d_patch_kernel");
     return IDE3D_OK;
 }
@@ -623,7 +586,7 @@ __global__ void __launch_bounds__(256) upfirdn2d_cl_patch_kernel(const UpfirArgs
 
 // TMA-staged channels_last flavour (C % 32 == 0): a block owns a 32 x 16 pixel output tile x 32 channels; the input box
 // (channels x columns x rows of a 4-D tensor map, zero-filled outside the image by the TMA unit) arrives with ONE
-// cp.async.bulk.tensor.4d per tile, double-buffered against the FIR of the previous tile.  Shared-memory pixels are 128-byte
+// tma_load_4d per tile, double-buffered against the FIR of the previous tile.  Shared-memory pixels are 128-byte
 // (fp32) runs of 32 channels, so the 8 lanes that share a patch read one contiguous line per window element.
 // Tile shapes: CB channels x (PX x PY patches of 4 x 4 pixels), CB/4 * PX * PY = 256 threads.  The TMA unit is fed one
 // innermost run (CB channels) per request, so wider channel blocks move more bytes per request: 64 channels x 16x16 pixels
@@ -645,11 +608,6 @@ struct ClTmaGeom {
     static constexpr int kSmem = kStages * kTileBytes + 128 + 128;
     static_assert(kCV * PX * PY == 256, "one thread per (channel vector, patch)");
 };
-__device__ __forceinline__ void tma_load_tile4(void* dst, const CUtensorMap* map, unsigned long long* bar, int c, int x, int y, int n, unsigned bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_addr(bar)), "r"(bytes) : "memory");
-    asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-                 ::"r"(smem_addr(dst)), "l"(map), "r"(smem_addr(bar)), "r"(c), "r"(x), "r"(y), "r"(n) : "memory");
-}
 template <typename T> struct V4s;
 template <> struct V4s<float> {
     static __device__ __forceinline__ void ld(const float* p, float (&o)[4]) { const float4 t = *reinterpret_cast<const float4*>(p); o[0] = t.x; o[1] = t.y; o[2] = t.z; o[3] = t.w; }
@@ -672,7 +630,7 @@ __global__ void __launch_bounds__(256, 2) upfirdn2d_cl_tma_kernel(const UpfirArg
     extern __shared__ unsigned char tma_raw[];
     unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(tma_raw) + 127) & ~(uintptr_t)127);
     constexpr int NST = GM::kStages;
-    unsigned long long* bars = reinterpret_cast<unsigned long long*>(base + NST * GM::kTileBytes);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(base + NST * GM::kTileBytes);
     float fk[FH][FW];
     load_filter<FW, FH>(p, fk);
     const int ax = floor_div(p.px0, UX), ay = floor_div(p.py0, UY);
@@ -689,12 +647,13 @@ __global__ void __launch_bounds__(256, 2) upfirdn2d_cl_tma_kernel(const UpfirArg
     auto issue = [&](long long t, int buf) {
         int n, cb, ox_t, oy_t;
         coords(t, n, cb, ox_t, oy_t);
-        tma_load_tile4(base + buf * GM::kTileBytes, &tmap, &bars[buf], cb * kClCB, ox_t * DX / UX - ax + AX::lo(),
-                       oy_t * DY / UY - ay + AY::lo(), n, kBytes);
+        const int c = cb * kClCB, x = ox_t * DX / UX - ax + AX::lo(), y = oy_t * DY / UY - ay + AY::lo();
+        mbar_arrive_expect_tx(&bars[buf], kBytes);
+        tma_load_4d(base + buf * GM::kTileBytes, &tmap, &bars[buf], c, x, y, n);
     };
     if (threadIdx.x == 0) {
-        for (int i = 0; i < NST; ++i) tma_bar_init(&bars[i]);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        for (int i = 0; i < NST; ++i) mbar_init(&bars[i], 1);
+        mbar_fence_init();
         for (int i = 0; i < NST; ++i)
             if ((long long)blockIdx.x + (long long)i * gridDim.x < total) issue((long long)blockIdx.x + (long long)i * gridDim.x, i);
     }
@@ -707,7 +666,7 @@ __global__ void __launch_bounds__(256, 2) upfirdn2d_cl_tma_kernel(const UpfirArg
         const int cur = it % NST;
         int n, cb, ox_t, oy_t;
         coords(t, n, cb, ox_t, oy_t);
-        tma_bar_wait(&bars[cur], (it / NST) & 1);
+        mbar_wait(&bars[cur], (it / NST) & 1);
         const T* tile = reinterpret_cast<const T*>(base + cur * GM::kTileBytes) + ((pty * AY::kStep) * GM::BW + ptx * AX::kStep) * kClCB + cvl * 4;
         const int ox0 = ox_t + ptx * kPatch, oy0 = oy_t + pty * kPatch;
         if (ox0 < p.out_w && oy0 < p.out_h)
@@ -732,7 +691,7 @@ static int launch_cl_tma(const UpfirArgs& p, cudaStream_t st_) {
     const CUresult r = encode_tiled()(&map, sizeof(T) == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4,
                                       const_cast<void*>(p.x), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                       CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) IDE3D_FAIL(IDE3D_UNSUPPORTED, "upfirdn2d: cuTensorMapEncodeTiled (channels_last) failed (%d)", (int)r);
+    if (r != CUDA_SUCCESS) IDE3D_FAIL(IDE3D_UNSUPPORTED, "upfirdn2d: encoding the channels_last tensor map failed (%d)", (int)r);
     void (*kern)(const UpfirArgs, int, int, int, const CUtensorMap) = p.epi ? upfirdn2d_cl_tma_kernel<T, UX, UY, DX, DY, FW, FH, PHX, PHY, kEpi, CB>
                                                                             : upfirdn2d_cl_tma_kernel<T, UX, UY, DX, DY, FW, FH, PHX, PHY, kPlain, CB>;
     if constexpr (std::is_same<T, __half>::value)
@@ -740,15 +699,10 @@ static int launch_cl_tma(const UpfirArgs& p, cudaStream_t st_) {
     if constexpr (std::is_same<T, float>::value)
         if (p.mixed) return IDE3D_UNSUPPORTED;                                  // the fp16 skip add runs in the L1-gather kernel
     const size_t smem = GM::kSmem;
-    if (smem > 48 * 1024) IDE3D_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int tiles_x = ceil_div(p.out_w, kClTileW), tiles_y = ceil_div(p.out_h, kClTileH), cblocks = p.in_c / kClCB;
-    const long long total = (long long)tiles_x * tiles_y * cblocks * p.in_n;
-    int per_sm = 1;
-    IDE3D_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, smem));
-    if (per_sm < 1) per_sm = 1;
-    long long grid = (long long)sm_count() * per_sm;
-    if (grid > total) grid = total;
-    kern<<<(unsigned)grid, 256, smem, st_>>>(p, tiles_x, tiles_y, cblocks, map);
+    int grid = 0, rc;
+    if ((rc = persistent_grid(kern, 256, smem, (long long)tiles_x * tiles_y * cblocks * p.in_n, grid)) != IDE3D_OK) return rc;
+    kern<<<grid, 256, smem, st_>>>(p, tiles_x, tiles_y, cblocks, map);
     IDE3D_CHECK_LAUNCH("upfirdn2d_cl_tma_kernel");
     return IDE3D_OK;
 }

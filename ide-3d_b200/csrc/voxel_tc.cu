@@ -47,8 +47,8 @@ __global__ void __launch_bounds__(kTcThreads) sigma_tc_kernel(const Args a) {
     const int W = a.seg.w, H = a.seg.h;
     unsigned char* a_hi = tile_base + wg * kStageBytes;
     unsigned char* a_lo = a_hi + kTileBytes;
-    const uint64_t ah = tc::make_sdesc_sw128(tc::smem_u32(a_hi)), al = tc::make_sdesc_sw128(tc::smem_u32(a_lo));
-    const uint64_t wh = tc::make_sdesc_sw128(tc::smem_u32(w_hi)), wl = tc::make_sdesc_sw128(tc::smem_u32(w_lo));
+    const uint64_t ah = tc::make_sdesc_sw128(smem_u32(a_hi)), al = tc::make_sdesc_sw128(smem_u32(a_lo));
+    const uint64_t wh = tc::make_sdesc_sw128(smem_u32(w_hi)), wl = tc::make_sdesc_sw128(smem_u32(w_lo));
     const float sig_b = a.b2[0];
     const long long stride = (long long)kWarpgroups * gridDim.x;
 

@@ -197,6 +197,19 @@ def test_raymarch_entry_points_share_validation(lib, case):
     assert lib.ide3d_last_error() == fwd_error
 
 
+@pytest.mark.skipif(torch.cuda.is_available(), reason='passes fake device pointers: run only where no GPU can be reached')
+@pytest.mark.parametrize('field', ['x_c', 'x_n', 'y_w', 'y_h'])
+def test_filtered_lrelu_rejects_empty_output(lib, field):
+    """ide3d_filtered_lrelu refuses a call with no output elements before anything reaches the device."""
+    p = _lib.FlreluParams()
+    p.x = p.fu = p.fd = p.y = 0x10000
+    p.dtype, p.up, p.down, p.fu_w, p.fd_w = _lib.F32, 2, 2, 12, 12
+    p.x_w = p.x_h = p.x_c = p.x_n = p.y_w = p.y_h = 4
+    setattr(p, field, 0)
+    assert lib.ide3d_filtered_lrelu(ctypes.byref(p), None) == _lib.INVALID
+    assert b'y is empty' in lib.ide3d_last_error()
+
+
 @pytest.mark.parametrize('option, error', [(dict(clamp_mode='bogus'), ValueError), (dict(fill_mode='bogus'), NotImplementedError)])
 def test_raymarch_backward_checks_options_like_forward(option, error):
     from ide3d_b200 import render
