@@ -259,6 +259,11 @@ SIGNATURES = {
     'ide3d_resample_u8': (_i32, [_vp, _i32, _i32, _i32, _i32, _i64, _i64, _i64, _vp, _i32, _i32, _i64, _i64, _i64, _i32, _vp, _vp, _i32,
                                  _vp, _vp, _vp, _i64, _vp]),
     'ide3d_style_grid': (_i32, [_vp, _i32, _i32, _i32, _i32, _i32, _i32, _i64, _i64, _i64, _i64, _vp, _i64, _i64, _vp]),
+    'ide3d_viz_image_scratch_bytes': (_i64, [_i32, _i32, _i32]),
+    'ide3d_viz_image': (_i32, [_vp, _i32, _i32, _i32, _i32, _i64, _i64, _i64, _i32, _i32, _i32, _i32, _f32, _vp, _i32, _i64, _i64, _i64,
+                               _vp, _vp, _i64, _vp]),
+    'ide3d_viz_fft_scratch_bytes': (_i64, [_i32, _i32, _i32]),
+    'ide3d_viz_fft': (_i32, [_vp, _i32, _i32, _i32, _i32, _i64, _i64, _i64, _vp, _f32, _vp, _i32, _vp, _i64, _i64, _i64, _vp, _i64, _vp]),
 }
 
 

@@ -19,7 +19,7 @@ OBJ = os.path.join(HERE, '_build_tuning' if os.environ.get('IDE3D_BUILD_TUNING',
 LIBDIR = os.path.join(HERE, 'lib')
 LIB = os.path.join(LIBDIR, 'libide3d_b200_tuning.so' if os.environ.get('IDE3D_BUILD_TUNING', '0') == '1' else 'libide3d_b200.so')
 TUNING = os.environ.get('IDE3D_BUILD_TUNING', '0') == '1'      # experiment switches (A/B scripts only)
-UNITS = ['capi', 'raymarch', 'raymarch_bwd', 'raymarch_tc', 'voxel', 'voxel_tc', 'stages', 'style_plan', 'mcubes', 'raster', 'frames', 'strips', 'projector', 'lpips', 'seg_stem', 'bias_act', 'upfirdn2d', 'filtered_lrelu', 'filtered_lrelu_fused', 'knn', 'spectra', 'resample', 'style_grid']
+UNITS = ['capi', 'raymarch', 'raymarch_bwd', 'raymarch_tc', 'voxel', 'voxel_tc', 'stages', 'style_plan', 'mcubes', 'raster', 'frames', 'strips', 'projector', 'lpips', 'seg_stem', 'bias_act', 'upfirdn2d', 'filtered_lrelu', 'filtered_lrelu_fused', 'knn', 'spectra', 'resample', 'style_grid', 'viz']
 NVCC_FLAGS = ['-O3', '-std=c++17', '--expt-relaxed-constexpr', '-gencode', 'arch=compute_90a,code=sm_90a',
               '-lineinfo', '-Xcompiler', '-fPIC', '-Xptxas', '-v'] + (['-DIDE3D_TUNING'] if TUNING else [])
 

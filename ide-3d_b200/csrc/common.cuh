@@ -83,6 +83,14 @@ inline int persistent_grid(Kernel kern, int threads, size_t smem, long long max_
     return IDE3D_OK;
 }
 
+// torch's float -> uint8 conversion on the device after (v * 127.5 + 128).clamp(0, 255): two rounded float ops, clamp lets NaN through,
+// and the cast goes float -> int64 -> uint8 (the conversion of save_image_u8 in strips.cu).
+__device__ __forceinline__ unsigned char torch_u8(float v) {
+    float y = __fadd_rn(__fmul_rn(v, 127.5f), 128.f);
+    if (y == y) y = fminf(fmaxf(y, 0.f), 255.f);
+    return (unsigned char)(long long)y;
+}
+
 // floor division for possibly negative numerators
 __host__ __device__ inline int floor_div(int a, int b) {
     int q = a / b;

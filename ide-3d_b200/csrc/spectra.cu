@@ -18,8 +18,9 @@
 //            ends in the half-plane spectrum [P / 2 + 1, P] (k2-major).  One owner per bin, images in order: no atomics, reruns
 //            are bit-identical, and the result does not depend on how the images are split into calls.
 //
-// Twiddles come from one table of w_P^j, j < P, built per CTA with sincospi (w_N^k = w_P^{interp k}); the CTAs are persistent.
-#include "common.cuh"
+// Twiddles come from one table of w_P^j, j < P, built per CTA with sincospi (w_N^k = w_P^{interp k}); the CTAs are persistent.  The FFT
+// itself is fft.cuh's, shared with the visualizer's FFT panel (viz.cu).
+#include "fft.cuh"
 
 namespace ide3d {
 namespace {
@@ -39,46 +40,13 @@ struct SpecArgs {
     int B, C, N, logN, I, logI, P, H, F, logF;
 };
 
-__device__ __forceinline__ double2 cmul(double2 a, double2 b) { return make_double2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
-
-__device__ __forceinline__ void twiddle_table(double2* tw, int P) {
-    for (int j = threadIdx.x; j < P; j += kThreads) {
-        double s, c;
-        sincospi(2.0 * j / P, &s, &c);
-        tw[j] = make_double2(c, -s);
-    }
-}
-
-// In-place radix-2 DIF over the tile: kTile / N sequences of length N at row stride N + 1; output in bit-reversed order.
-__device__ __forceinline__ void dif_fft(double2* buf, const double2* tw, const SpecArgs& a) {
-    const int N = a.N, half = N >> 1, logHalf = a.logN - 1;
-    for (int logh = a.logN - 1; logh >= 0; --logh) {
-        const int h = 1 << logh;
-        const int tstep = a.P >> (logh + 1);                 // w_N^{j N / 2h} = w_P^{j P / 2h}
-#pragma unroll
-        for (int k = 0; k < kPer / 2; ++k) {
-            const int t = threadIdx.x + k * kThreads;
-            const int f = t >> logHalf, q = t & (half - 1);
-            const int j = q & (h - 1);
-            const int i = ((q >> logh) << (logh + 1)) + j;
-            double2* p = buf + f * (N + 1) + i;
-            const double2 x = p[0], y = p[h];
-            p[0] = make_double2(x.x + y.x, x.y + y.y);
-            p[h] = cmul(make_double2(x.x - y.x, x.y - y.y), tw[j * tstep]);
-        }
-        __syncthreads();
-    }
-}
-
-__device__ __forceinline__ int bitrev(int m, int logN) { return (int)(__brev((unsigned)m) >> (32 - logN)); }
-
 __global__ void __launch_bounds__(kThreads) spectrum_rows_kernel(SpecArgs a) {
     extern __shared__ double2 spec_smem[];
     double2* tw = spec_smem;                               // [P]
     double2* buf = tw + a.P;                               // [F, N + 1]
     double* lut = reinterpret_cast<double*>(buf + a.F * (a.N + 1));    // [256]
     double* win = lut + 256;                               // [N]
-    twiddle_table(tw, a.P);
+    twiddle_table<kThreads>(tw, a.P);
     for (int j = threadIdx.x; j < 256; j += kThreads) lut[j] = a.lut[j];
     for (int j = threadIdx.x; j < a.N; j += kThreads) win[j] = a.window[j];
     __syncthreads();
@@ -108,7 +76,7 @@ __global__ void __launch_bounds__(kThreads) spectrum_rows_kernel(SpecArgs a) {
             buf[f * (N + 1) + n2] = v;
         }
         __syncthreads();
-        dif_fft(buf, tw, a);
+        dif_fft<kThreads, kTile>(buf, tw, a.N, a.logN, a.P);
         // m <= N / 2 is all the half plane k2 = I m + r <= P / 2 needs
         const int outs = a.F * (N / 2 + 1);
         for (int e = threadIdx.x; e < outs; e += kThreads) {
@@ -131,7 +99,7 @@ __global__ void __launch_bounds__(kThreads) spectrum_cols_kernel(SpecArgs a) {
     extern __shared__ double2 spec_smem[];
     double2* tw = spec_smem;
     double2* buf = tw + a.P;
-    twiddle_table(tw, a.P);
+    twiddle_table<kThreads>(tw, a.P);
     __syncthreads();
 
     const int N = a.N;
@@ -166,7 +134,7 @@ __global__ void __launch_bounds__(kThreads) spectrum_cols_kernel(SpecArgs a) {
                     buf[f * (N + 1) + n1] = v;
                 }
                 __syncthreads();
-                dif_fft(buf, tw, a);
+                dif_fft<kThreads, kTile>(buf, tw, a.N, a.logN, a.P);
 #pragma unroll
                 for (int k = 0; k < kPer; ++k) {
                     const int e = threadIdx.x + k * kThreads;
@@ -228,12 +196,6 @@ __global__ void __launch_bounds__(256) image_moments_kernel(const uint8_t* __res
         atomicAdd(moments + 1, s1);
         atomicAdd(moments + 2, s2);
     }
-}
-
-int log2_exact(int v) {
-    int l = 0;
-    while ((1 << l) < v) ++l;
-    return (1 << l) == v ? l : -1;
 }
 
 // IDE3D_UNSUPPORTED for a shape the kernels do not cover, IDE3D_OK otherwise

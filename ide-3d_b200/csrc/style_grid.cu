@@ -8,14 +8,6 @@ namespace ide3d {
 
 constexpr int kGridTileX = 64, kGridTileY = 4;      // 256 threads, one canvas pixel each
 
-// torch's (img * 127.5 + 128).clamp(0, 255).to(torch.uint8) on the device: two rounded float ops, clamp lets NaN through, and the cast
-// goes float -> int64 -> uint8 (the conversion of save_image_u8 in strips.cu).
-__device__ __forceinline__ unsigned char style_mix_u8(float v) {
-    float y = __fadd_rn(__fmul_rn(v, 127.5f), 128.f);
-    if (y == y) y = fminf(fmaxf(y, 0.f), 255.f);
-    return (unsigned char)(long long)y;
-}
-
 __global__ void __launch_bounds__(kGridTileX * kGridTileY)
 style_grid_kernel(const float* __restrict__ cells, int first_row, int cols, int views, int height, int width, long long first_cell,
                   long long stride_n, long long stride_c, long long stride_h, long long stride_w, unsigned char* __restrict__ out,
@@ -33,7 +25,7 @@ style_grid_kernel(const float* __restrict__ cells, int first_row, int cols, int 
     const long long n = (slot - 1 - first_cell) * views + v;
     const float* im = cells + n * stride_n + yy * stride_h + xx * stride_w;
 #pragma unroll
-    for (int c = 0; c < 3; ++c) o[c] = style_mix_u8(__ldg(im + c * stride_c));
+    for (int c = 0; c < 3; ++c) o[c] = torch_u8(__ldg(im + c * stride_c));
 }
 
 }  // namespace ide3d

@@ -391,12 +391,14 @@ class SynthesisBlock(torch.nn.Module):
         needs the chained path below): premodulated_x -- x already carries conv0's styles (the previous block's epilogue wrote
         them); x_next_styles [N, C] -- return `x * x_next_styles` (the next block's conv0 styles) instead of x; drop_x -- return
         no x (nothing consumes it); fp16_operands -- run the convolutions on fp16 operands (fp16_operands(); needs the style plan's
-        dcoefs for that path).  y_rgb is the ToRGB output (bias included) when conv1's epilogue computed it."""
+        dcoefs for that path); unlinked -- run every layer on its own (no chaining).  y_rgb is the ToRGB output (bias included) when
+        conv1's epilogue computed it."""
         layer_kwargs = dict(layer_kwargs)
         premod_in = layer_kwargs.pop('premodulated_x', False)
         x_next_styles = layer_kwargs.pop('x_next_styles', None)
         drop_x = layer_kwargs.pop('drop_x', False)
         fp16 = layer_kwargs.pop('fp16_operands', False)
+        unlinked = layer_kwargs.pop('unlinked', False)
         misc.assert_shape(ws, [None, self.num_conv + self.num_torgb, self.w_dim])
         w_iter = iter(ws.unbind(dim=1))
         dtype = torch.float16 if self.use_fp16 and not force_fp32 else torch.float32
@@ -410,7 +412,8 @@ class SynthesisBlock(torch.nn.Module):
             fused_modconv = fused_modconv and self.resolution >= thr
         # Inference in fp32 with activation scaling: every epilogue also writes the next layer's `x * styles`, so the
         # separate modulation passes of conv1 and ToRGB disappear (conv0 -> x*s1 only; conv1 -> x and x*s_rgb).
-        chain = CHAIN_MODULATION and (not fused_modconv) and dtype == torch.float32 and not (torch.is_grad_enabled() and (
+        # unlinked (SynthesisNetwork.forward): every layer returns its own output, as forward hooks expect
+        chain = CHAIN_MODULATION and not unlinked and (not fused_modconv) and dtype == torch.float32 and not (torch.is_grad_enabled() and (
             ws.requires_grad or any(p.requires_grad for p in self.parameters())))
         if not chain and (premod_in or x_next_styles is not None or drop_x):
             raise RuntimeError('SynthesisBlock: cross-block chaining needs the chained fp32 inference path')

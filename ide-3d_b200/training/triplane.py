@@ -309,21 +309,10 @@ class SynthesisNetwork(torch.nn.Module):
             x, rgb = block(x, rgb, cur_ws, **kw)
         return rgb
 
-    def forward(self, ws, c=None, render_params=None, noise_mode='const', force_fp32=False, return_seg=False,
-                return_raw=False, return_dict=False, fused_modconv=None, views=1, shared_prefix=None, **render_overrides):
-        """views (extension): render every latent from `views` cameras with ONE backbone pass.  ws [N, num_ws, w_dim]; c [N * views, 25]
-        in latent-major order (row i * views + j is view j of latent i); every output has N * views rows in that order.  The
-        tri-plane backbone runs on the N latents, the renderer and the super-resolution blocks per view (their ws repeated per view).
-        seed= (a render override) may then hold N * views per-frame jitter seeds.
-        shared_prefix (extension) = (k, groups): groups holds N host ints, and latents with equal ids have equal ws rows for the first k
-        backbone blocks (prefix_blocks gives k for a set of differing rows).  Those k blocks then run once per group, on the group's first
-        latent, with the plain call's arithmetic, and their outputs are repeated per latent; the other blocks run per latent.  Only the
-        prefix blocks' batch changes, and with it possibly cuDNN's algorithm choice.  Nothing shared (k == 0 or all ids distinct) is
-        the plain call."""
-        views = int(views)
-        if views < 1:
-            raise ValueError(f'SynthesisNetwork: views must be >= 1, got {views}')
-        voxel_ws, block_ws = self.split_ws(ws)
+    def planes(self, ws, noise_mode='const', force_fp32=False, fused_modconv=None, shared_prefix=None, unlinked=False):
+        """The tri-plane backbone of a synthesis call: -> (img_v, seg_v, style plan | None).  The plan holds every layer's styles and
+        demodulation coefficients of the call; render_planes reads its super-resolution rows.  Arguments as forward's."""
+        voxel_ws, _ = self.split_ws(ws)
         if shared_prefix is not None:
             k, groups = int(shared_prefix[0]), np.asarray(shared_prefix[1]).reshape(-1)
             if not 0 <= k <= len(self.voxel_block_resolutions) or groups.shape[0] != ws.shape[0]:
@@ -333,25 +322,45 @@ class SynthesisNetwork(torch.nn.Module):
             shared_prefix = None if k == 0 or len(first) == len(groups) else \
                 (k, torch.from_numpy(first).to(ws.device), torch.from_numpy(inverse.reshape(-1)).to(ws.device))
         block_kwargs = dict(noise_mode=noise_mode, force_fp32=force_fp32, fused_modconv=fused_modconv)
-        # fp16 convolution operands in the tri-plane backbone only: the super-resolution blocks write the image itself, and there one
-        # more rounding per convolution moves frames rendered at different batch sizes apart by 2 uint8 levels
-        # (tests/test_gpu_multiview.py allows 1)
-        backbone = [getattr(self, f'vb{r}') for r in self.voxel_block_resolutions]
-        fp16 = networks.fp16_operands(backbone, force_fp32=force_fp32, fused_modconv=fused_modconv)
-        plan = self._style_plan(ws, fp16_blocks=backbone if fp16 else ())
-        sr_kwargs = dict(block_kwargs)
-        if plan is not None:
-            block_kwargs['style_plan'] = sr_kwargs['style_plan'] = plan
-            if fp16:
-                block_kwargs['fp16_operands'] = True
+        plan = None
+        if unlinked:
+            block_kwargs['unlinked'] = True
+        else:
+            # fp16 convolution operands in the tri-plane backbone only: the super-resolution blocks write the image itself, and there
+            # one more rounding per convolution moves frames rendered at different batch sizes apart by 2 uint8 levels
+            # (tests/test_gpu_multiview.py allows 1)
+            backbone = [getattr(self, f'vb{r}') for r in self.voxel_block_resolutions]
+            fp16 = networks.fp16_operands(backbone, force_fp32=force_fp32, fused_modconv=fused_modconv)
+            plan = self._style_plan(ws, fp16_blocks=backbone if fp16 else ())
+            if plan is not None:
+                block_kwargs['style_plan'] = plan
+                if fp16:
+                    block_kwargs['fp16_operands'] = True
         img_v, seg_v = self.backbone(voxel_ws, shared_prefix=shared_prefix, **block_kwargs)
+        return img_v, seg_v, plan
+
+    def render_planes(self, img_v, seg_v, ws, c=None, render_params=None, noise_mode='const', force_fp32=False, return_seg=False,
+                      return_raw=False, return_dict=False, fused_modconv=None, views=1, style_plan=None, unlinked=False,
+                      **render_overrides):
+        """Everything of a synthesis call after the backbone: the renderer and the super-resolution blocks, from the planes `planes`
+        returned for these ws.  style_plan: the plan `planes` returned (its super-resolution rows are read).  The other arguments and
+        the outputs are forward's; forward is planes followed by this call."""
+        views = int(views)
+        if views < 1:
+            raise ValueError(f'SynthesisNetwork: views must be >= 1, got {views}')
+        _, block_ws = self.split_ws(ws)
+        sr_kwargs = dict(noise_mode=noise_mode, force_fp32=force_fp32, fused_modconv=fused_modconv)
+        if unlinked:
+            sr_kwargs['unlinked'] = True
+        elif style_plan is not None:
+            sr_kwargs['style_plan'] = style_plan
         if views > 1:
             # the per-view part: SR styles are functions of the ws row alone, so the plan's rows are repeated rather than recomputed
             block_ws = [w.repeat_interleave(views, 0) for w in block_ws]
-            if plan is not None:
+            if 'style_plan' in sr_kwargs:
                 rep = lambda t: None if t is None else t.repeat_interleave(views, 0)
                 sr_layers = {m for r in self.block_resolutions for m in getattr(self, f'b{r}').modules()}
-                sr_kwargs['style_plan'] = {layer: (rep(st), rep(dc)) for layer, (st, dc) in plan.items() if layer in sr_layers}
+                sr_kwargs['style_plan'] = {layer: (rep(st), rep(dc)) for layer, (st, dc) in style_plan.items() if layer in sr_layers}
 
         kw = dict(self.rendering_kwargs)
         kw.update({k: v for k, v in (render_params or {}).items() if k in ('fov', 'num_steps', 'ray_start', 'ray_end',
@@ -391,6 +400,28 @@ class SynthesisNetwork(torch.nn.Module):
         if return_raw:
             return img, feat_img[:, :self.img_channels]
         return img
+
+    def forward(self, ws, c=None, render_params=None, noise_mode='const', force_fp32=False, return_seg=False,
+                return_raw=False, return_dict=False, fused_modconv=None, views=1, shared_prefix=None, unlinked=False, **render_overrides):
+        """views (extension): render every latent from `views` cameras with ONE backbone pass.  ws [N, num_ws, w_dim]; c [N * views, 25]
+        in latent-major order (row i * views + j is view j of latent i); every output has N * views rows in that order.  The
+        tri-plane backbone runs on the N latents, the renderer and the super-resolution blocks per view (their ws repeated per view).
+        seed= (a render override) may then hold N * views per-frame jitter seeds.
+        shared_prefix (extension) = (k, groups): groups holds N host ints, and latents with equal ids have equal ws rows for the first k
+        backbone blocks (prefix_blocks gives k for a set of differing rows).  Those k blocks then run once per group, on the group's first
+        latent, with the plain call's arithmetic, and their outputs are repeated per latent; the other blocks run per latent.  Only the
+        prefix blocks' batch changes, and with it possibly cuDNN's algorithm choice.  Nothing shared (k == 0 or all ids distinct) is
+        the plain call.
+        unlinked (extension): every layer computes its own styles and returns its own output, and every block returns its x -- no style
+        plan, no `x * styles` written for the next layer, no fp16 operands.  What forward hooks need to see each layer's output
+        (viz.renderer's layer capture); the chained default computes the same function with fewer passes."""
+        if int(views) < 1:
+            raise ValueError(f'SynthesisNetwork: views must be >= 1, got {views}')
+        img_v, seg_v, plan = self.planes(ws, noise_mode=noise_mode, force_fp32=force_fp32, fused_modconv=fused_modconv,
+                                         shared_prefix=shared_prefix, unlinked=unlinked)
+        return self.render_planes(img_v, seg_v, ws, c=c, render_params=render_params, noise_mode=noise_mode, force_fp32=force_fp32,
+                                  return_seg=return_seg, return_raw=return_raw, return_dict=return_dict, fused_modconv=fused_modconv,
+                                  views=views, style_plan=plan, unlinked=unlinked, **render_overrides)
 
 
 # ================================================================================================ generator

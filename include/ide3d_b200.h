@@ -45,6 +45,10 @@
  *   ide3d_image_moments       avg_spectra.py:126-131  `stats`: sums of 1, x and x^2, as exact integers
  *   ide3d_resample_u8         dataset_tool.py:226-256  PIL.Image.resize(LANCZOS) of 8-bit L / RGB images (Pillow's ImagingResample)
  *   ide3d_style_grid          apps/style_mixing.py:100-153  the uint8 conversion and the canvas paste loop of the style-mixing grid
+ *   ide3d_viz_image           viz/renderer.py:369-393  the display tail: statistics, depth normalisation, channel window, inf-norm, dB gain,
+ *                             uint8 image
+ *   ide3d_viz_fft             viz/renderer.py:395-406  the FFT panel: mean removal, Kaiser window, |2-D DFT|^2 over channels, roll, dB,
+ *                             colormap
  *
  * Conventions
  *   - plain C: raw device pointers, sizes, strides (in ELEMENTS), a cudaStream_t passed as void*.
@@ -771,6 +775,35 @@ int ide3d_resample_u8(const uint8_t* in, int n, int c, int in_h, int in_w, int64
 int ide3d_style_grid(const float* cells, int first_row, int rows, int cols, int views, int height, int width, int64_t stride_n,
                      int64_t stride_c, int64_t stride_h, int64_t stride_w, uint8_t* out, int64_t out_stride_row, int64_t out_stride_view,
                      ide3d_stream_t stream);
+
+/* The display tail of viz/renderer.py:369-393 for one map x [c, h, w], float32 (dtype IDE3D_F32) or float16 (IDE3D_F16, widened
+ * exactly as .to(torch.float32) does), element strides.  sel = channels [base_channel, base_channel + sel_channels).
+ *   stats float32 [6] (or null) = mean, unbiased std and inf-norm of x, then of sel, from float64 sums of the raw values.
+ *   out: byte (y, x, j) at out + y * out_stride_h + x * out_stride_w + j * out_stride_c for j < out_channels, from selected channel
+ *   min(j, sel_channels - 1), in torch's float32 operations and order: with depth, v = ((v - min x) / fl(max x - min x) - 0.5) * -2
+ *   (min and max over the whole map); with normalize, v / clip(max |v| over its channel, 1e-8, 1e8); v * gain; then
+ *   (v * 127.5 + 128).clamp(0, 255) -> uint8.  The bytes equal torch's on the device.
+ * Two launches, deterministic: a float64 reduction into one partial per CTA, then the elementwise pass, which folds the partials in a
+ * fixed order.  scratch: ide3d_viz_image_scratch_bytes(c, h, w) bytes, 16-byte aligned.  IDE3D_INVALID for bad shapes, a window outside
+ * [0, c), normalize with more than 1024 selected channels, null pointers or too little scratch, decided before any launch. */
+int64_t ide3d_viz_image_scratch_bytes(int c, int h, int w);
+int ide3d_viz_image(const void* x, int dtype, int c, int h, int w, int64_t stride_c, int64_t stride_h, int64_t stride_w, int base_channel,
+                    int sel_channels, int depth, int normalize, float gain, uint8_t* out, int out_channels, int64_t out_stride_h,
+                    int64_t out_stride_w, int64_t out_stride_c, float* stats, void* scratch, int64_t scratch_bytes, ide3d_stream_t stream);
+
+/* The FFT panel of viz/renderer.py:396-406 for a map x [c, n, n] (float32 or float16, element strides), in float64:
+ *     P[k1, k2] = sum_c |DFT2((x_c - mean x_c) * window[n1] window[n2])[k1, k2]|^2,
+ * rolled by n / 2 in both axes, index = clamp(floor(((10 log10(P / mean P) / range_db + 1) / 2) * (lut_size - 1) + 0.5), 0, lut_size - 1),
+ * and the panel pixel (y, x) gets lut[index] (uint8 [lut_size, 3]) at out + y * out_stride_h + x * out_stride_w + j * out_stride_c.  A
+ * zero bin (-inf dB) and a constant map (mean P = 0) give index 0.  window: float64 [n], torch.kaiser_window(n, periodic=False, beta).
+ * The FFT is fft.cuh's radix-2 transform, rows (half plane) then columns; the channel sum and the mean run in a fixed order, so reruns
+ * are bit-identical.  scratch: ide3d_viz_fft_scratch_bytes(c, h, w) bytes, 256-byte aligned.  IDE3D_UNSUPPORTED unless h == w is a
+ * power of two in [4, 1024] (the caller falls back to the reference's arithmetic); IDE3D_INVALID for c < 1, null pointers or too little
+ * scratch.  Every check runs before any launch. */
+int64_t ide3d_viz_fft_scratch_bytes(int c, int h, int w);
+int ide3d_viz_fft(const void* x, int dtype, int c, int h, int w, int64_t stride_c, int64_t stride_h, int64_t stride_w, const double* window,
+                  float range_db, const uint8_t* lut, int lut_size, uint8_t* out, int64_t out_stride_h, int64_t out_stride_w,
+                  int64_t out_stride_c, void* scratch, int64_t scratch_bytes, ide3d_stream_t stream);
 
 #ifdef __cplusplus
 }
