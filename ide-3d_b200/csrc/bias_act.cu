@@ -6,6 +6,7 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "elem.cuh"
 
 namespace ide3d {
 
@@ -16,9 +17,6 @@ struct BiasActArgs {
     float alpha, gain, clamp;
     long long size_x, size_b, step_b;
 };
-
-template <typename T> struct Acc { using type = float; };
-template <> struct Acc<double> { using type = double; };
 
 template <typename S> __device__ __forceinline__ S exp_(S v);
 template <> __device__ __forceinline__ float exp_<float>(float v) { return __expf(v); }
@@ -88,59 +86,6 @@ __device__ __forceinline__ long long bias_index(long long e, const BiasActArgs& 
     return (e / p.step_b) % p.size_b;
 }
 
-template <typename T> struct Vec;
-template <> struct Vec<float> { static constexpr int N = 4; using type = float4; };
-template <> struct Vec<__half> { static constexpr int N = 8; using type = uint4; };
-template <> struct Vec<double> { static constexpr int N = 2; using type = double2; };
-
-template <typename T> __device__ __forceinline__ typename Acc<T>::type to_acc(T v) { return (typename Acc<T>::type)v; }
-template <> __device__ __forceinline__ float to_acc<__half>(__half v) { return __half2float(v); }
-template <typename T> __device__ __forceinline__ T from_acc(typename Acc<T>::type v) { return (T)v; }
-template <> __device__ __forceinline__ __half from_acc<__half>(float v) { return __float2half(v); }
-
-// one 16-byte vector <-> N accumulator-typed registers (explicit unpacking: no local-memory round trip)
-__device__ __forceinline__ void load_vec(const float* p, long long v, float (&o)[4]) {
-    const float4 t = __ldcs(reinterpret_cast<const float4*>(p) + v);
-    o[0] = t.x; o[1] = t.y; o[2] = t.z; o[3] = t.w;
-}
-__device__ __forceinline__ void load_vec(const double* p, long long v, double (&o)[2]) {
-    const double2 t = __ldcs(reinterpret_cast<const double2*>(p) + v);
-    o[0] = t.x; o[1] = t.y;
-}
-__device__ __forceinline__ void load_vec(const __half* p, long long v, float (&o)[8]) {
-    const uint4 t = __ldcs(reinterpret_cast<const uint4*>(p) + v);
-    const unsigned w[4] = {t.x, t.y, t.z, t.w};
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[i]));
-        o[2 * i] = f.x; o[2 * i + 1] = f.y;
-    }
-}
-__device__ __forceinline__ void load_vec(const __half* p, long long v, float (&o)[4]) {
-    const uint2 t = __ldcs(reinterpret_cast<const uint2*>(p) + v);
-    const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&t.x)), b = __half22float2(*reinterpret_cast<const __half2*>(&t.y));
-    o[0] = a.x; o[1] = a.y; o[2] = b.x; o[3] = b.y;
-}
-__device__ __forceinline__ void store_vec(float* p, long long v, const float (&o)[4]) {
-    __stcs(reinterpret_cast<float4*>(p) + v, make_float4(o[0], o[1], o[2], o[3]));
-}
-__device__ __forceinline__ void store_vec(double* p, long long v, const double (&o)[2]) {
-    __stcs(reinterpret_cast<double2*>(p) + v, make_double2(o[0], o[1]));
-}
-__device__ __forceinline__ void store_vec(__half* p, long long v, const float (&o)[4]) {    // 4 channels, rounded once each
-    const __half2 a = __floats2half2_rn(o[0], o[1]), b = __floats2half2_rn(o[2], o[3]);
-    __stcs(reinterpret_cast<uint2*>(p) + v, make_uint2(*reinterpret_cast<const unsigned*>(&a), *reinterpret_cast<const unsigned*>(&b)));
-}
-__device__ __forceinline__ void store_vec(__half* p, long long v, const float (&o)[8]) {
-    unsigned w[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const __half2 h = __floats2half2_rn(o[2 * i], o[2 * i + 1]);
-        w[i] = *reinterpret_cast<const unsigned*>(&h);
-    }
-    __stcs(reinterpret_cast<uint4*>(p) + v, make_uint4(w[0], w[1], w[2], w[3]));
-}
-
 // Vectorised kernel: every thread handles whole 16-byte vectors; the tail (size_x % N) is scalar.
 // Bias addressing per vector: BMODE 0 = none, 1 = one bias for the whole vector (step_b % N == 0: NCHW),
 // 2 = consecutive biases (step_b == 1 and size_b % N == 0: channels_last / [M, C] matrices), 3 = per element.
@@ -165,7 +110,7 @@ __global__ void __launch_bounds__(256) bias_act_kernel(const BiasActArgs p, cons
 #pragma unroll
         for (int u = 0; u < UNROLL; ++u) {
             const long long v = v0 + u * stride;
-            if (v < nvec) load_vec(x, v, vx[u]);                              // all loads of the unrolled group first
+            if (v < nvec) load_vec_cs(x, v, vx[u]);                           // all loads of the unrolled group first
         }
 #pragma unroll
         for (int u = 0; u < UNROLL; ++u) {
@@ -173,9 +118,9 @@ __global__ void __launch_bounds__(256) bias_act_kernel(const BiasActArgs p, cons
             if (v >= nvec) continue;
             const long long e0 = v * N;
             S exr[N], eyr[N], edy[N], out[N], bb[N];
-            if (xref) load_vec(xref, v, exr);
-            if (yref) load_vec(yref, v, eyr);
-            if (dy) load_vec(dy, v, edy);
+            if (xref) load_vec_cs(xref, v, exr);
+            if (yref) load_vec_cs(yref, v, eyr);
+            if (dy) load_vec_cs(dy, v, edy);
             if (bmode == 1) {
                 const S t = to_acc<T>(b[bias_index(e0, p, small)]);
 #pragma unroll
@@ -191,7 +136,7 @@ __global__ void __launch_bounds__(256) bias_act_kernel(const BiasActArgs p, cons
 #pragma unroll
             for (int j = 0; j < N; ++j)
                 out[j] = eval<S, A>(vx[u][j], bb[j], xref ? exr[j] : (S)0, yref ? eyr[j] : (S)0, dy ? edy[j] : (S)1, G, alpha, gain, clamp);
-            store_vec(y, v, out);
+            store_vec_cs(y, v, out);
         }
     }
     // scalar tail
@@ -224,20 +169,20 @@ __global__ void __launch_bounds__(256) bias_act_planar_kernel(const BiasActArgs 
         S vx[UNROLL][N];
 #pragma unroll
         for (int u = 0; u < UNROLL; ++u)
-            if (v0 + u * 256 < plane_vecs) load_vec((const T*)p.x, vbase + v0 + u * 256, vx[u]);
+            if (v0 + u * 256 < plane_vecs) load_vec_cs((const T*)p.x, vbase + v0 + u * 256, vx[u]);
 #pragma unroll
         for (int u = 0; u < UNROLL; ++u) {
             const long long vi = v0 + u * 256;
             if (vi >= plane_vecs) continue;
             const long long v = vbase + vi;
             S exr[N], eyr[N], edy[N], out[N];
-            if (p.xref) load_vec((const T*)p.xref, v, exr);
-            if (p.yref) load_vec((const T*)p.yref, v, eyr);
-            if (p.dy) load_vec((const T*)p.dy, v, edy);
+            if (p.xref) load_vec_cs((const T*)p.xref, v, exr);
+            if (p.yref) load_vec_cs((const T*)p.yref, v, eyr);
+            if (p.dy) load_vec_cs((const T*)p.dy, v, edy);
 #pragma unroll
             for (int j = 0; j < N; ++j)
                 out[j] = eval<S, A>(vx[u][j], bias, p.xref ? exr[j] : (S)0, p.yref ? eyr[j] : (S)0, p.dy ? edy[j] : (S)1, G, alpha, gain, clamp);
-            store_vec((T*)p.y, v, out);
+            store_vec_cs((T*)p.y, v, out);
         }
     }
 }
@@ -246,11 +191,6 @@ template <typename T, int A>
 static int launch_bias_act(const BiasActArgs& p, cudaStream_t st) {
     constexpr int UNROLL = 4;
     constexpr int N = Vec<T>::N;
-    const long long nvec = p.size_x / N;
-    long long blocks = ceil_div<long long>(nvec > 0 ? nvec : 1, 256ll * UNROLL);
-    const long long cap = (long long)sm_count() * 8;            // 8 resident blocks of 256 threads per SM
-    if (blocks > cap) blocks = cap;
-    if (blocks < 1) blocks = 1;
     int bmode = 0;
     if (p.b != nullptr) bmode = (p.step_b % N == 0) ? 1 : ((p.step_b == 1 && p.size_b % N == 0) ? 2 : 3);
     // planar fast path: whole planes of >= 1024 elements share one bias (or there is no bias at all)
@@ -258,14 +198,15 @@ static int launch_bias_act(const BiasActArgs& p, cudaStream_t st) {
     if ((p.b == nullptr || bmode == 1) && plane_elems >= 1024 && plane_elems % N == 0 && p.size_x % plane_elems == 0) {
         const long long cpp = ceil_div<long long>(plane_elems / N, 256ll * UNROLL);
         const long long items = (p.size_x / plane_elems) * cpp;
-        long long g = items < cap ? items : cap;
-        if (p.grad == 0) bias_act_planar_kernel<T, A, UNROLL, true><<<(unsigned)g, 256, 0, st>>>(p, plane_elems, cpp, items);
-        else bias_act_planar_kernel<T, A, UNROLL, false><<<(unsigned)g, 256, 0, st>>>(p, plane_elems, cpp, items);
+        const unsigned g = capped_grid(items, 8);                   // 8 resident blocks of 256 threads per SM
+        if (p.grad == 0) bias_act_planar_kernel<T, A, UNROLL, true><<<g, 256, 0, st>>>(p, plane_elems, cpp, items);
+        else bias_act_planar_kernel<T, A, UNROLL, false><<<g, 256, 0, st>>>(p, plane_elems, cpp, items);
         IDE3D_CHECK_LAUNCH("bias_act_planar_kernel");
         return IDE3D_OK;
     }
-    if (p.grad == 0) bias_act_kernel<T, A, UNROLL, true><<<(unsigned)blocks, 256, 0, st>>>(p, bmode);
-    else bias_act_kernel<T, A, UNROLL, false><<<(unsigned)blocks, 256, 0, st>>>(p, bmode);
+    const unsigned blocks = capped_grid(ceil_div<long long>(p.size_x / N, 256ll * UNROLL), 8);
+    if (p.grad == 0) bias_act_kernel<T, A, UNROLL, true><<<blocks, 256, 0, st>>>(p, bmode);
+    else bias_act_kernel<T, A, UNROLL, false><<<blocks, 256, 0, st>>>(p, bmode);
     IDE3D_CHECK_LAUNCH("bias_act_kernel");
     return IDE3D_OK;
 }
@@ -328,25 +269,6 @@ struct EpiArgs {
     int noise_batch;                      // 1: one noise map for the whole batch, n: one per sample
 };
 
-template <typename T> __device__ __forceinline__ void load_vec_keep(const T* p, long long v, typename Acc<T>::type (&o)[Vec<T>::N]);
-template <> __device__ __forceinline__ void load_vec_keep<float>(const float* p, long long v, float (&o)[4]) {
-    const float4 t = __ldg(reinterpret_cast<const float4*>(p) + v);
-    o[0] = t.x; o[1] = t.y; o[2] = t.z; o[3] = t.w;
-}
-template <> __device__ __forceinline__ void load_vec_keep<double>(const double* p, long long v, double (&o)[2]) {
-    const double2 t = __ldg(reinterpret_cast<const double2*>(p) + v);
-    o[0] = t.x; o[1] = t.y;
-}
-template <> __device__ __forceinline__ void load_vec_keep<__half>(const __half* p, long long v, float (&o)[8]) {
-    const uint4 t = __ldg(reinterpret_cast<const uint4*>(p) + v);
-    const unsigned w[4] = {t.x, t.y, t.z, t.w};
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[i]));
-        o[2 * i] = f.x; o[2 * i + 1] = f.y;
-    }
-}
-
 // NCHW: (plane, chunk) work items, scale and bias are block-uniform, the noise map is read through L1/L2 (it is shared by
 // every channel of the sample).
 template <typename T, int A, int UNROLL>
@@ -369,8 +291,8 @@ __global__ void __launch_bounds__(256) modconv_epilogue_planar_kernel(const EpiA
 #pragma unroll
         for (int u = 0; u < UNROLL; ++u)
             if (v0 + u * 256 < plane_vecs) {
-                load_vec((const T*)p.x, vbase + v0 + u * 256, vx[u]);
-                if (p.noise) load_vec_keep<T>((const T*)p.noise, nbase + v0 + u * 256, vn[u]);
+                load_vec_cs((const T*)p.x, vbase + v0 + u * 256, vx[u]);
+                if (p.noise) load_vec_ro((const T*)p.noise, nbase + v0 + u * 256, vn[u]);
             }
 #pragma unroll
         for (int u = 0; u < UNROLL; ++u) {
@@ -382,11 +304,11 @@ __global__ void __launch_bounds__(256) modconv_epilogue_planar_kernel(const EpiA
                 const S t = p.noise ? vx[u][j] * d + vn[u][j] : vx[u][j] * d;
                 out[j] = eval<S, A>(t, bias, (S)0, (S)0, (S)1, 0, alpha, gain, clamp);
             }
-            if (p.y) store_vec((T*)p.y, vbase + vi, out);
+            if (p.y) store_vec_cs((T*)p.y, vbase + vi, out);
             if (p.y2) {
 #pragma unroll
                 for (int j = 0; j < N; ++j) out[j] *= d2;
-                store_vec((T*)p.y2, vbase + vi, out);
+                store_vec_cs((T*)p.y2, vbase + vi, out);
             }
         }
     }
@@ -412,7 +334,7 @@ __global__ void __launch_bounds__(256) modconv_epilogue_cl_kernel(const EpiArgs 
         S vx[UNROLL][N];
 #pragma unroll
         for (int u = 0; u < UNROLL; ++u)
-            if (v0 + u * 256u < svec) load_vec((const T*)p.x, vbase + v0 + u * 256u, vx[u]);
+            if (v0 + u * 256u < svec) load_vec_cs((const T*)p.x, vbase + v0 + u * 256u, vx[u]);
 #pragma unroll
         for (int u = 0; u < UNROLL; ++u) {
             const unsigned vi = v0 + u * 256u;
@@ -421,8 +343,8 @@ __global__ void __launch_bounds__(256) modconv_epilogue_cl_kernel(const EpiArgs 
             if (cv_shift >= 0) { pix = vi >> cv_shift; c0 = vi & (cv - 1u); }
             else { pix = vi / cv; c0 = vi - pix * cv; }
             S d[N], bb[N], out[N];
-            if (p.scale) load_vec_keep<T>((const T*)p.scale, (long long)smp * cv + c0, d);
-            if (p.b) load_vec_keep<T>((const T*)p.b, c0, bb);
+            if (p.scale) load_vec_ro((const T*)p.scale, (long long)smp * cv + c0, d);
+            if (p.b) load_vec_ro((const T*)p.b, c0, bb);
             const S nz = p.noise ? to_acc<T>(__ldg((const T*)p.noise + (p.noise_batch == 1 ? (long long)pix : (long long)smp * p.hw + pix))) : (S)0;
 #pragma unroll
             for (int j = 0; j < N; ++j) {
@@ -430,13 +352,13 @@ __global__ void __launch_bounds__(256) modconv_epilogue_cl_kernel(const EpiArgs 
                 if (p.noise) t = p.scale ? vx[u][j] * d[j] + nz : vx[u][j] + nz;
                 out[j] = eval<S, A>(t, p.b ? bb[j] : (S)0, (S)0, (S)0, (S)1, 0, alpha, gain, clamp);
             }
-            if (p.y) store_vec((TO*)p.y, vbase + vi, out);
+            if (p.y) store_vec_cs((TO*)p.y, vbase + vi, out);
             if (p.y2) {
                 S d2[N];
-                load_vec_keep<T>((const T*)p.scale2, (long long)smp * cv + c0, d2);
+                load_vec_ro((const T*)p.scale2, (long long)smp * cv + c0, d2);
 #pragma unroll
                 for (int j = 0; j < N; ++j) out[j] *= d2[j];
-                store_vec((TO*)p.y2, vbase + vi, out);
+                store_vec_cs((TO*)p.y2, vbase + vi, out);
             }
         }
     }
@@ -446,18 +368,16 @@ template <typename T, typename TO, int A>
 static int launch_epilogue(const EpiArgs& p, int channels_last, cudaStream_t st) {
     constexpr int UNROLL = 4;
     constexpr int N = Vec<T>::N;
-    const long long cap = (long long)sm_count() * 8;
     if (channels_last) {
         if (p.c % N != 0) IDE3D_FAIL(IDE3D_UNSUPPORTED, "modconv_epilogue: channels_last needs C %% %d == 0", N);
         const long long svec = p.hw * (p.c / N);
         if (svec >= (1ll << 31)) IDE3D_FAIL(IDE3D_UNSUPPORTED, "modconv_epilogue: more than 2^31 vectors per sample");
         const long long cps = ceil_div<long long>(svec, 256ll * UNROLL);
         const long long items = p.n * cps;
-        const long long blocks = items < cap ? items : cap;
         const long long cvn = p.c / N;
         int cv_shift = -1;
         if ((cvn & (cvn - 1)) == 0) { cv_shift = 0; while ((1ll << cv_shift) < cvn) ++cv_shift; }
-        modconv_epilogue_cl_kernel<T, TO, A, UNROLL><<<(unsigned)blocks, 256, 0, st>>>(p, (unsigned)cps, items, cv_shift);
+        modconv_epilogue_cl_kernel<T, TO, A, UNROLL><<<capped_grid(items, 8), 256, 0, st>>>(p, (unsigned)cps, items, cv_shift);
         IDE3D_CHECK_LAUNCH("modconv_epilogue_cl_kernel");
         return IDE3D_OK;
     }
@@ -465,8 +385,7 @@ static int launch_epilogue(const EpiArgs& p, int channels_last, cudaStream_t st)
     if (p.hw % N != 0) IDE3D_FAIL(IDE3D_UNSUPPORTED, "modconv_epilogue: H*W must be a multiple of %d", N);
     const long long cpp = ceil_div<long long>(p.hw / N, 256ll * UNROLL);
     const long long items = p.n * p.c * cpp;
-    const long long g = items < cap ? items : cap;
-    modconv_epilogue_planar_kernel<T, A, UNROLL><<<(unsigned)g, 256, 0, st>>>(p, cpp, items);
+    modconv_epilogue_planar_kernel<T, A, UNROLL><<<capped_grid(items, 8), 256, 0, st>>>(p, cpp, items);
     IDE3D_CHECK_LAUNCH("modconv_epilogue_planar_kernel");
     return IDE3D_OK;
 }
@@ -545,11 +464,6 @@ struct EpiRgbArgs {
     int noise_batch;
 };
 
-__device__ __forceinline__ void load4(const float* p, long long v, float (&o)[4]) {
-    const float4 t = __ldg(reinterpret_cast<const float4*>(p) + v);
-    o[0] = t.x; o[1] = t.y; o[2] = t.z; o[3] = t.w;
-}
-
 template <typename T, int A, bool kShfl>
 __global__ void __launch_bounds__(256) modconv_epilogue_rgb_cl_kernel(const EpiRgbArgs p, int ppb, unsigned chunks_per_sample,
                                                                      long long items) {
@@ -570,10 +484,10 @@ __global__ void __launch_bounds__(256) modconv_epilogue_rgb_cl_kernel(const EpiR
             const long long sv = (long long)smp * cv + c0;
 #pragma unroll
             for (int j = 0; j < 4; ++j) d[j] = bb[j] = ys[j] = s2[j] = 1.f;
-            if (p.scale) load4(p.scale, sv, d);
-            if (p.b) load4(p.b, c0, bb);
-            if (p.yscale) load4(p.yscale, sv, ys);
-            if (p.y2) load4(p.scale2, sv, s2);
+            if (p.scale) load_vec_ro(p.scale, sv, d);
+            if (p.b) load_vec_ro(p.b, c0, bb);
+            if (p.yscale) load_vec_ro(p.yscale, sv, ys);
+            if (p.y2) load_vec_ro(p.scale2, sv, s2);
 #pragma unroll
             for (int o = 0; o < kRgbMax; ++o)
 #pragma unroll
@@ -588,7 +502,7 @@ __global__ void __launch_bounds__(256) modconv_epilogue_rgb_cl_kernel(const EpiR
 #pragma unroll
         for (int u = 0; u < UNROLL; ++u) {
             const unsigned pix = pix0 + u * ppb + lp;
-            if (lane_on && pix < (unsigned)p.hw) load_vec((const T*)p.x, vbase + pix * cv + c0, vx[u]);
+            if (lane_on && pix < (unsigned)p.hw) load_vec_cs((const T*)p.x, vbase + pix * cv + c0, vx[u]);
         }
 #pragma unroll
         for (int u = 0; u < UNROLL; ++u) {
@@ -608,12 +522,12 @@ __global__ void __launch_bounds__(256) modconv_epilogue_rgb_cl_kernel(const EpiR
                 if (p.y) {
 #pragma unroll
                     for (int j = 0; j < 4; ++j) out[j] = p.yscale ? t[j] * ys[j] : t[j];
-                    store_vec((T*)p.y, v, out);
+                    store_vec_cs((T*)p.y, v, out);
                 }
                 if (p.y2) {
 #pragma unroll
                     for (int j = 0; j < 4; ++j) out[j] = t[j] * s2[j];
-                    store_vec((T*)p.y2, v, out);
+                    store_vec_cs((T*)p.y2, v, out);
                 }
                 if (want_rgb) {
 #pragma unroll
@@ -657,10 +571,9 @@ static int launch_epilogue_rgb(const EpiRgbArgs& p, cudaStream_t st) {
     const int ppb = 256 / cv;
     const long long cps = ceil_div<long long>(p.hw, (long long)ppb * UNROLL);
     const long long items = (long long)p.n * cps;
-    const long long cap = (long long)sm_count() * 8;
-    const long long blocks = items < cap ? items : cap;
-    if (shfl) modconv_epilogue_rgb_cl_kernel<T, A, true><<<(unsigned)blocks, 256, 0, st>>>(p, ppb, (unsigned)cps, items);
-    else modconv_epilogue_rgb_cl_kernel<T, A, false><<<(unsigned)blocks, 256, 0, st>>>(p, ppb, (unsigned)cps, items);
+    const unsigned blocks = capped_grid(items, 8);
+    if (shfl) modconv_epilogue_rgb_cl_kernel<T, A, true><<<blocks, 256, 0, st>>>(p, ppb, (unsigned)cps, items);
+    else modconv_epilogue_rgb_cl_kernel<T, A, false><<<blocks, 256, 0, st>>>(p, ppb, (unsigned)cps, items);
     IDE3D_CHECK_LAUNCH("modconv_epilogue_rgb_cl_kernel");
     return IDE3D_OK;
 }

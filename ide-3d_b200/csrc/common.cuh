@@ -83,6 +83,14 @@ inline int persistent_grid(Kernel kern, int threads, size_t smem, long long max_
     return IDE3D_OK;
 }
 
+// Grid of a grid-stride kernel: one CTA per work item, at most `per_sm` CTAs per SM, at least one.  Work items are blocks of
+// threads (the caller's ceil_div) or the items a kernel loops over with its CTAs.
+inline unsigned capped_grid(long long work_items, int per_sm) {
+    long long grid = (long long)sm_count() * per_sm;
+    if (work_items < grid) grid = work_items;
+    return (unsigned)(grid < 1 ? 1 : grid);
+}
+
 // torch's float -> uint8 conversion on the device after (v * 127.5 + 128).clamp(0, 255): two rounded float ops, clamp lets NaN through,
 // and the cast goes float -> int64 -> uint8 (the conversion of save_image_u8 in strips.cu).
 __device__ __forceinline__ unsigned char torch_u8(float v) {

@@ -12,6 +12,8 @@
 // (backward gradient is 0; clamp wins over sign).  Filters are kernel arguments / shared memory here, never
 // global __constant__ state, so concurrent streams are safe (the reference is not: filtered_lrelu.cu:77-78).
 #include "common.cuh"
+#include "elem.cuh"
+#include "filtered_lrelu.cuh"
 
 namespace ide3d {
 
@@ -23,11 +25,6 @@ struct ActArgs {
     int sw, sh, sox, soy;
     float gain, slope, clamp;
 };
-
-template <typename T> __device__ __forceinline__ float ldf(const T* p) { return (float)(*p); }
-template <> __device__ __forceinline__ float ldf<__half>(const __half* p) { return __half2float(*p); }
-template <typename T> __device__ __forceinline__ void stf(T* p, float v) { *p = (T)v; }
-template <> __device__ __forceinline__ void stf<__half>(__half* p, float v) { *p = __float2half(v); }
 
 // MODE 0: plain forward, 1: write signs, 2: read signs.  One thread per element in x; a 16-lane group
 // owns one 32-bit word of the sign tensor (16 elements * 2 bits).
@@ -51,10 +48,10 @@ __global__ void __launch_bounds__(256) lrelu_act_kernel(const ActArgs p) {
         if (MODE == 1) {
             unsigned s = 0;
             if (x < p.xw && y < p.xh) {
-                float v = ldf<T>(pv) * p.gain;
+                float v = load_f32<T>(pv) * p.gain;
                 if (v < 0.f) { v *= p.slope; s = 1; }
                 if (fabsf(v) > p.clamp) { v = (v < 0.f) ? -p.clamp : p.clamp; s = 2; }
-                stf<T>(pv, v);
+                store_f32<T>(pv, v);
             }
             s <<= (lane16 << 1);
             const unsigned m = (threadIdx.x & 16) ? 0xffff0000u : 0x0000ffffu;
@@ -67,7 +64,7 @@ __global__ void __launch_bounds__(256) lrelu_act_kernel(const ActArgs p) {
                 reinterpret_cast<unsigned*>(p.s)[is >> 4] = s;
             }
         } else if (x < p.xw) {
-            float v = ldf<T>(pv) * p.gain;
+            float v = load_f32<T>(pv) * p.gain;
             if (MODE == 2) {
                 const unsigned sx = (unsigned)(x + p.sox), sy = (unsigned)(y + p.soy);
                 if (sx < (unsigned)p.sw && sy < (unsigned)p.sh) {
@@ -81,7 +78,7 @@ __global__ void __launch_bounds__(256) lrelu_act_kernel(const ActArgs p) {
                 if (v < 0.f) v *= p.slope;
                 if (fabsf(v) > p.clamp) v = (v < 0.f) ? -p.clamp : p.clamp;
             }
-            stf<T>(pv, v);
+            store_f32<T>(pv, v);
         }
     }
 }
@@ -90,13 +87,10 @@ template <typename T>
 static int launch_act(const ActArgs& a, int write_signs, int read_signs, cudaStream_t st) {
     const int width = write_signs ? a.sw : a.xw, height = write_signs ? a.sh : a.xh;
     const long long total = (long long)a.xc * a.xn * height * ((width + 15) >> 4) * 16;
-    long long grid = ceil_div<long long>(total, 256);
-    const long long cap = (long long)sm_count() * 16;
-    if (grid > cap) grid = cap;
-    if (grid < 1) grid = 1;
-    if (write_signs) lrelu_act_kernel<T, 1><<<(unsigned)grid, 256, 0, st>>>(a);
-    else if (read_signs) lrelu_act_kernel<T, 2><<<(unsigned)grid, 256, 0, st>>>(a);
-    else lrelu_act_kernel<T, 0><<<(unsigned)grid, 256, 0, st>>>(a);
+    const unsigned grid = capped_grid(ceil_div<long long>(total, 256), 16);
+    if (write_signs) lrelu_act_kernel<T, 1><<<grid, 256, 0, st>>>(a);
+    else if (read_signs) lrelu_act_kernel<T, 2><<<grid, 256, 0, st>>>(a);
+    else lrelu_act_kernel<T, 0><<<grid, 256, 0, st>>>(a);
     IDE3D_CHECK_LAUNCH("lrelu_act_kernel");
     return IDE3D_OK;
 }
@@ -132,24 +126,6 @@ extern "C" int ide3d_filtered_lrelu_act(const ide3d_filtered_lrelu_act_params* q
     }
     IDE3D_FAIL(IDE3D_INVALID, "filtered_lrelu_act: unsupported dtype %d", q->dtype);
 }
-
-// ------------------------------------------------------------------------------------------------------------
-// Fused kernel for separable filters: filtered_lrelu_fused.cu
-namespace ide3d {
-struct FlFusedArgs {
-    const void* x; const void* b; const float* fu; const float* fd; void* y; unsigned char* s;
-    int px0, py0, flip;
-    float gain, slope, clamp;
-    int xw, xh, xc, xn;
-    long long sxw, sxh, sxc, sxn;
-    int yw, yh;
-    long long syw, syh, syc, syn;
-    int sw, sh, sox, soy, mode;
-    int one_u, one_d;
-    int channels_last;
-};
-int launch_filtered_lrelu_fused(const FlFusedArgs& a, int dtype, int up, int down, int fu, int fd, cudaStream_t st);
-}  // namespace ide3d
 
 extern "C" int ide3d_filtered_lrelu(const ide3d_filtered_lrelu_params* q, ide3d_stream_t stream) {
     IDE3D_REQUIRE(q && q->x && q->y && q->fu && q->fd, "filtered_lrelu: null tensor");

@@ -27,31 +27,13 @@
 // number of leading samples to skip (< UP).  Loops run over blocks of P input samples, P chosen so that every ring slot, filter
 // phase, down-sampling phase and sign-nibble position is a compile-time constant inside the unrolled block body.
 #include "common.cuh"
+#include "elem.cuh"
+#include "filtered_lrelu.cuh"
 #include "tma.cuh"
 
 namespace ide3d {
 
-struct FlFusedArgs {
-    const void* x; const void* b; const float* fu; const float* fd; void* y; unsigned char* s;
-    int px0, py0, flip;
-    float gain, slope, clamp;
-    int xw, xh, xc, xn;
-    long long sxw, sxh, sxc, sxn;
-    int yw, yh;
-    long long syw, syh, syc, syn;
-    int sw, sh, sox, soy, mode;          // mode 0: plain, 1: write signs, 2: read signs
-    int one_u, one_d;                    // 1x1 "full" filters carry their value once, not once per axis
-    int channels_last;
-};
-
 namespace flf {
-
-template <typename T> __device__ __forceinline__ float ldf(const T* p) { return (float)(*p); }
-template <> __device__ __forceinline__ float ldf<__half>(const __half* p) { return __half2float(*p); }
-template <typename T> __device__ __forceinline__ void stf(T* p, float v) { *p = (T)v; }
-template <> __device__ __forceinline__ void stf<__half>(__half* p, float v) { *p = __float2half(v); }
-template <typename T> __device__ __forceinline__ T zero_of() { return (T)0.f; }
-template <> __device__ __forceinline__ __half zero_of<__half>() { return __float2half(0.f); }
 
 __host__ __device__ constexpr int cgcd(int a, int b) { return b == 0 ? a : cgcd(b, a % b); }
 __host__ __device__ constexpr int clcm(int a, int b) { return a / cgcd(a, b) * b; }
@@ -303,7 +285,7 @@ filtered_lrelu_fused2_kernel(const FlFusedArgs p, int tiles_x, int tiles_y, int 
                 const int x = r2 % G::IW, seg = r2 / G::IW;
                 const int gx = ix_t + x, gc = c0 + c;
                 const bool colok = (unsigned)gx < (unsigned)p.xw && gc < p.xc;
-                const float bias = (colok && p.b) ? ldf<T>((const T*)p.b + gc) : 0.f;
+                const float bias = (colok && p.b) ? load_f32<T>((const T*)p.b + gc) : 0.f;
                 const int j0 = seg * G::RA;                                   // first intermediate row of the segment
                 const int e0 = phy + j0;
                 const int b0 = (e0 + UP - 1) / UP;
@@ -315,7 +297,7 @@ filtered_lrelu_fused2_kernel(const FlFusedArgs p, int tiles_x, int tiles_y, int 
 #pragma unroll
                 for (int t = 0; t < TU - 1; ++t) {
                     const bool ok = colok && (unsigned)(iy_t + b0 + t) < (unsigned)p.xh;
-                    hw[t] = ldf<T>(col + (long long)t * G::BW * CB) + (ok ? bias : 0.f);
+                    hw[t] = load_f32<T>(col + (long long)t * G::BW * CB) + (ok ? bias : 0.f);
                 }
 #pragma unroll 1
                 for (int bk = 0; bk < G::NB_A; ++bk) {
@@ -323,7 +305,7 @@ filtered_lrelu_fused2_kernel(const FlFusedArgs p, int tiles_x, int tiles_y, int 
                     for (int ii = 0; ii < P; ++ii) {
                         const int ip = bk * P + ii;
                         const bool ok = colok && (unsigned)(iy_t + b0 + TU - 1 + ip) < (unsigned)p.xh;
-                        hw[(TU - 1 + ii) % TU] = ldf<T>(col + (long long)(TU - 1 + ip) * G::BW * CB) + (ok ? bias : 0.f);
+                        hw[(TU - 1 + ii) % TU] = load_f32<T>(col + (long long)(TU - 1 + ip) * G::BW * CB) + (ok ? bias : 0.f);
 #pragma unroll
                         for (int m = 0; m < UP; ++m) {
                             const int r = UP - 1 - m;
@@ -401,7 +383,7 @@ filtered_lrelu_fused2_kernel(const FlFusedArgs p, int tiles_x, int tiles_y, int 
 #pragma unroll
                                 for (int k = 0; k < FD; ++k) o = fmaf(fdv[k], uw[(ii + 1 + k) % FD], o);
                                 const int oy = oy_t + o0 + num / DOWN;
-                                if (colok && oy < p.yh) stf<T>(yc + (long long)oy * p.syh, o);
+                                if (colok && oy < p.yh) store_f32<T>(yc + (long long)oy * p.syh, o);
                             }
                         }
                     }

@@ -72,10 +72,7 @@ extern "C" int ide3d_mc_classify(const float* volume, int nx, int ny, int nz, fl
     IDE3D_REQUIRE(volume && ntri_table && counts, "mc_classify: null argument");
     IDE3D_REQUIRE(nx >= 2 && ny >= 2 && nz >= 2, "mc_classify: the grid needs at least 2 points per axis");
     const long long cells = (long long)(nx - 1) * (ny - 1) * (nz - 1);
-    long long grid = ceil_div<long long>(cells, 256);
-    const long long cap = (long long)sm_count() * 16;
-    if (grid > cap) grid = cap;
-    mc_classify_kernel<<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(volume, nx, ny, nz, threshold, ntri_table, counts);
+    mc_classify_kernel<<<capped_grid(ceil_div<long long>(cells, 256), 16), 256, 0, (cudaStream_t)stream>>>(volume, nx, ny, nz, threshold, ntri_table, counts);
     IDE3D_CHECK_LAUNCH("mc_classify_kernel");
     return IDE3D_OK;
 }
@@ -86,12 +83,10 @@ extern "C" int ide3d_mc_emit(const float* volume, int nx, int ny, int nz, float 
     IDE3D_REQUIRE(volume && tri_table && edge_corner && counts && offsets && edge_ids && verts, "mc_emit: null argument");
     IDE3D_REQUIRE(nx >= 2 && ny >= 2 && nz >= 2, "mc_emit: the grid needs at least 2 points per axis");
     const long long cells = (long long)(nx - 1) * (ny - 1) * (nz - 1);
-    long long grid = ceil_div<long long>(cells, 256);
-    const long long cap = (long long)sm_count() * 16;
-    if (grid > cap) grid = cap;
-    mc_emit_kernel<<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(volume, nx, ny, nz, threshold, tri_table, edge_corner, counts,
-                                                                      reinterpret_cast<const long long*>(offsets),
-                                                                      reinterpret_cast<long long*>(edge_ids), verts);
+    const unsigned grid = capped_grid(ceil_div<long long>(cells, 256), 16);
+    mc_emit_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(volume, nx, ny, nz, threshold, tri_table, edge_corner, counts,
+                                                           reinterpret_cast<const long long*>(offsets),
+                                                           reinterpret_cast<long long*>(edge_ids), verts);
     IDE3D_CHECK_LAUNCH("mc_emit_kernel");
     return IDE3D_OK;
 }

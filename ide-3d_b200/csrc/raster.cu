@@ -247,13 +247,6 @@ __global__ void __launch_bounds__(256) raster_resolve_kernel(const int* __restri
     }
 }
 
-inline unsigned grid_for(long long n, int block, int per_sm) {
-    long long g = ceil_div<long long>(n, block);
-    const long long cap = (long long)sm_count() * per_sm;
-    if (g > cap) g = cap;
-    return (unsigned)(g < 1 ? 1 : g);
-}
-
 }  // namespace ide3d
 
 using namespace ide3d;
@@ -269,8 +262,9 @@ extern "C" int ide3d_mesh_normals(const float* vertices, const int32_t* triangle
     IDE3D_REQUIRE(num_vertices >= 0, "mesh_normals: negative vertex count");
     if (num_vertices == 0) return IDE3D_OK;
     IDE3D_REQUIRE(vertices && triangles && adj_offsets && adj_faces && normals, "mesh_normals: null argument");
-    mesh_normals_kernel<<<grid_for(num_vertices, 256, 16), 256, 0, (cudaStream_t)stream>>>(vertices, triangles, num_vertices, adj_offsets,
-                                                                                          adj_faces, normals);
+    const unsigned grid = capped_grid(ceil_div<long long>(num_vertices, 256), 16);
+    mesh_normals_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(vertices, triangles, num_vertices, adj_offsets,
+                                                                adj_faces, normals);
     IDE3D_CHECK_LAUNCH("mesh_normals_kernel");
     return IDE3D_OK;
 }
@@ -305,20 +299,23 @@ extern "C" int ide3d_raster(const ide3d_raster_params* p, ide3d_stream_t stream)
     const double fyd = 1.0 / tan(0.5 * ((double)p->yfov_deg * (3.141592653589793 / 180.0)));
     const float fy = (float)fyd, fx = (float)(fyd * H / W);
 
-    raster_clear_kernel<<<grid_for(npix, 256, 16), 256, 0, s>>>(keys, npix, ocount);
+    const unsigned pix_grid = capped_grid(ceil_div<long long>(npix, 256), 16);
+    raster_clear_kernel<<<pix_grid, 256, 0, s>>>(keys, npix, ocount);
     IDE3D_CHECK_LAUNCH("raster_clear_kernel");
     if (p->num_triangles > 0) {
-        raster_transform_kernel<<<grid_for((long long)F * p->num_vertices, 256, 16), 256, 0, s>>>(p->vertices, p->num_vertices, p->cam2world,
-                                                                                                  F, W, H, fx, fy, p->znear, sv);
+        const unsigned vgrid = capped_grid(ceil_div<long long>((long long)F * p->num_vertices, 256), 16);
+        raster_transform_kernel<<<vgrid, 256, 0, s>>>(p->vertices, p->num_vertices, p->cam2world,
+                                                      F, W, H, fx, fy, p->znear, sv);
         IDE3D_CHECK_LAUNCH("raster_transform_kernel");
-        raster_small_kernel<<<grid_for((long long)F * p->num_triangles, 128, 32), 128, 0, s>>>(p->triangles, p->num_triangles, p->num_vertices,
-                                                                                               sv, F, W, H, keys, ocount, olist);
+        const unsigned tgrid = capped_grid(ceil_div<long long>((long long)F * p->num_triangles, 128), 32);
+        raster_small_kernel<<<tgrid, 128, 0, s>>>(p->triangles, p->num_triangles, p->num_vertices,
+                                                  sv, F, W, H, keys, ocount, olist);
         IDE3D_CHECK_LAUNCH("raster_small_kernel");
         raster_large_kernel<<<(unsigned)sm_count() * 4, 256, 0, s>>>(p->triangles, p->num_vertices, sv, W, H, keys, ocount, olist);
         IDE3D_CHECK_LAUNCH("raster_large_kernel");
     }
-    raster_resolve_kernel<<<grid_for(npix, 256, 16), 256, 0, s>>>(p->triangles, p->num_vertices, p->normals, sv, p->cam2world, F, W, H, p->base,
-                                                                  p->ambient, p->diffuse, p->background, keys, p->rgb, p->ids);
+    raster_resolve_kernel<<<pix_grid, 256, 0, s>>>(p->triangles, p->num_vertices, p->normals, sv, p->cam2world, F, W, H, p->base,
+                                                   p->ambient, p->diffuse, p->background, keys, p->rgb, p->ids);
     IDE3D_CHECK_LAUNCH("raster_resolve_kernel");
     return IDE3D_OK;
 }

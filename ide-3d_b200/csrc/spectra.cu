@@ -287,9 +287,8 @@ extern "C" int ide3d_image_moments(const uint8_t* images, int n, int c, int h, i
     if (n == 0) return IDE3D_OK;
     IDE3D_REQUIRE(images != nullptr, "image_moments: null images pointer");
     const int64_t rows = (int64_t)n * c * h;
-    const unsigned grid = (unsigned)(rows < 4LL * sm_count() ? rows : 4LL * sm_count());
-    image_moments_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(images, c, h, w, rows, stride_n, stride_c, stride_h, stride_w,
-                                                                 reinterpret_cast<unsigned long long*>(moments));
+    image_moments_kernel<<<capped_grid(rows, 4), 256, 0, (cudaStream_t)stream>>>(images, c, h, w, rows, stride_n, stride_c, stride_h, stride_w,
+                                                                                 reinterpret_cast<unsigned long long*>(moments));
     IDE3D_CHECK_LAUNCH("image_moments_kernel");
     return IDE3D_OK;
 }

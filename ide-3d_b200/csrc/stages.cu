@@ -217,14 +217,6 @@ __global__ void __launch_bounds__(256) pdf_kernel(const float* __restrict__ bins
     }
 }
 
-static inline unsigned grid_for(long long threads_needed, int block) {
-    long long g = ceil_div<long long>(threads_needed, block);
-    const long long cap = (long long)sm_count() * 16;
-    if (g > cap) g = cap;
-    if (g < 1) g = 1;
-    return (unsigned)g;
-}
-
 }  // namespace ide3d
 
 using namespace ide3d;
@@ -236,8 +228,9 @@ extern "C" int ide3d_initial_rays(int n, int num_steps, float fov_deg, int res_w
     IDE3D_REQUIRE(points && z_vals && rays_d_cam, "initial_rays: null output");
     const float cam_z = (float)(-1.0 / tan((2.0 * 3.14159265358979323846 * (double)fov_deg / 360.0) / 2.0));
     const long long total = (long long)n * res_w * res_h * num_steps;
-    rays_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(n, num_steps, cam_z, res_w, res_h, ray_start,
-                                                                      ray_end, points, z_vals, rays_d_cam);
+    const unsigned grid = capped_grid(ceil_div<long long>(total, 256), 16);
+    rays_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(n, num_steps, cam_z, res_w, res_h, ray_start,
+                                                        ray_end, points, z_vals, rays_d_cam);
     IDE3D_CHECK_LAUNCH("rays_kernel");
     return IDE3D_OK;
 }
@@ -249,7 +242,7 @@ extern "C" int ide3d_transform_points(const float* points, const float* z_vals, 
     IDE3D_REQUIRE(points && z_vals && dirs && cam2world && points_world && z_out && dirs_world && origins,
                   "transform_points: null pointer");
     const long long total = (long long)n * num_rays * num_steps;
-    transform_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(
+    transform_kernel<<<capped_grid(ceil_div<long long>(total, 256), 16), 256, 0, (cudaStream_t)stream>>>(
         points, z_vals, dirs, u, cam2world, n, num_rays, num_steps, points_world, z_out, dirs_world, origins);
     IDE3D_CHECK_LAUNCH("transform_kernel");
     return IDE3D_OK;
@@ -267,8 +260,9 @@ extern "C" int ide3d_sample_triplane(const ide3d_triplane* planes, const float* 
     const bool cl = planes->stride_c == 1 && planes->stride_w % 4 == 0 && planes->stride_h % 4 == 0 &&
                     planes->stride_n % 4 == 0 && (reinterpret_cast<uintptr_t>(planes->data) & 15) == 0;
     const long long threads = (long long)planes->n * num_points * 8;
-    if (cl) triplane_kernel<true><<<grid_for(threads, 256), 256, 0, (cudaStream_t)stream>>>(v, coords, planes->n, num_points, out);
-    else triplane_kernel<false><<<grid_for(threads, 256), 256, 0, (cudaStream_t)stream>>>(v, coords, planes->n, num_points, out);
+    const unsigned grid = capped_grid(ceil_div<long long>(threads, 256), 16);
+    if (cl) triplane_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(v, coords, planes->n, num_points, out);
+    else triplane_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(v, coords, planes->n, num_points, out);
     IDE3D_CHECK_LAUNCH("triplane_kernel");
     return IDE3D_OK;
 }
@@ -281,7 +275,7 @@ extern "C" int ide3d_integrate(const float* rgb_sigma, const float* rays_d_cam, 
     IDE3D_REQUIRE(n > 0 && num_rays > 0 && num_steps > 0 && channels >= 1, "integrate: empty request");
     IDE3D_REQUIRE(rgb_sigma && rays_d_cam && z_vals && rgb && depth && weights, "integrate: null pointer");
     const long long rays = (long long)n * num_rays;
-    integrate_kernel<<<grid_for(rays * 32, 256), 256, 0, (cudaStream_t)stream>>>(
+    integrate_kernel<<<capped_grid(ceil_div<long long>(rays * 32, 256), 16), 256, 0, (cudaStream_t)stream>>>(
         rgb_sigma, rays_d_cam, z_vals, (noise_std != 0.f) ? noise : nullptr, noise_std, rays, num_steps, channels,
         clamp_mode, last_back, white_back, max_depth, fill_weight, rgb, depth, weights);
     IDE3D_CHECK_LAUNCH("integrate_kernel");
@@ -296,9 +290,7 @@ extern "C" int ide3d_sample_pdf(const float* bins, const float* weights, const f
     const int warps = 8;
     const size_t smem = (size_t)warps * (num_bins + 1) * sizeof(float);
     IDE3D_REQUIRE(smem <= 48 * 1024, "sample_pdf: too many bins for one block");
-    unsigned grid = (unsigned)ceil_div(num_rays, warps);
-    const unsigned cap = (unsigned)sm_count() * 8;
-    if (grid > cap) grid = cap;
+    const unsigned grid = capped_grid(ceil_div(num_rays, warps), 8);
     pdf_kernel<<<grid, warps * 32, smem, (cudaStream_t)stream>>>(bins, weights, u, num_rays, num_bins, n_importance,
                                                                 eps, samples);
     IDE3D_CHECK_LAUNCH("pdf_kernel");
@@ -335,12 +327,10 @@ extern "C" int ide3d_mask2color(const float* masks, int n, int c, int h, int w, 
     const long long total = (long long)n * h * w;
     if (total == 0) return IDE3D_OK;
     IDE3D_REQUIRE(masks && lut && out, "mask2color: null tensor");
-    long long grid = ide3d::ceil_div<long long>(total, 256);
-    const long long cap = (long long)ide3d::sm_count() * 16;
-    if (grid > cap) grid = cap;
+    const unsigned grid = ide3d::capped_grid(ide3d::ceil_div<long long>(total, 256), 16);
     cudaStream_t st = (cudaStream_t)stream;
-    if (out_u8) ide3d::mask2color_kernel<unsigned char><<<(unsigned)grid, 256, 0, st>>>(masks, c, h, w, stride_n, stride_c, stride_h, stride_w, lut, (unsigned char*)out, total);
-    else ide3d::mask2color_kernel<float><<<(unsigned)grid, 256, 0, st>>>(masks, c, h, w, stride_n, stride_c, stride_h, stride_w, lut, (float*)out, total);
+    if (out_u8) ide3d::mask2color_kernel<unsigned char><<<grid, 256, 0, st>>>(masks, c, h, w, stride_n, stride_c, stride_h, stride_w, lut, (unsigned char*)out, total);
+    else ide3d::mask2color_kernel<float><<<grid, 256, 0, st>>>(masks, c, h, w, stride_n, stride_c, stride_h, stride_w, lut, (float*)out, total);
     IDE3D_CHECK_LAUNCH("mask2color_kernel");
     return IDE3D_OK;
 }

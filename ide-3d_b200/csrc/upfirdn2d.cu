@@ -18,6 +18,7 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "elem.cuh"
 #include "tma.cuh"
 
 namespace ide3d {
@@ -46,13 +47,6 @@ struct UpfirArgs {
     const void *scale = nullptr, *noise = nullptr, *scale2 = nullptr;
     void* y2 = nullptr;
 };
-
-template <typename T> struct AccT { using type = float; };
-template <> struct AccT<double> { using type = double; };
-template <typename T> __device__ __forceinline__ typename AccT<T>::type ld(const T* p) { return (typename AccT<T>::type)(*p); }
-template <> __device__ __forceinline__ float ld<__half>(const __half* p) { return __half2float(*p); }
-template <typename T> __device__ __forceinline__ void st(T* p, typename AccT<T>::type v) { *p = (T)v; }
-template <> __device__ __forceinline__ void st<__half>(__half* p, float v) { *p = __float2half(v); }
 
 // ------------------------------------------------------------------------------------------
 // compile-time polyphase bookkeeping for one axis: U = up, D = down, F = taps, PH = pad0 mod U
@@ -86,8 +80,8 @@ struct Axis {
 // 4x4 output patch of this thread from the staged input tile (row pitch PITCH), polyphase indices all compile-time
 template <typename T, typename TT, int UX, int UY, int DX, int DY, int FW, int FH, int PHX, int PHY, int PITCH>
 __device__ __forceinline__ void patch_compute_store_impl(const UpfirArgs& p, const TT* __restrict__ tile,
-                                                         const typename AccT<T>::type (&fk)[FH][FW], int n, int c, int ox_t, int oy_t) {
-    using S = typename AccT<T>::type;
+                                                         const typename Acc<T>::type (&fk)[FH][FW], int n, int c, int ox_t, int oy_t) {
+    using S = typename Acc<T>::type;
     using AX = Axis<UX, DX, FW, PHX>;
     using AY = Axis<UY, DY, FH, PHY>;
     constexpr int TIWP = PITCH;
@@ -103,7 +97,7 @@ __device__ __forceinline__ void patch_compute_store_impl(const UpfirArgs& p, con
     for (int r = 0; r < AY::kWin; ++r) {
         S win[AX::kWin];
 #pragma unroll
-        for (int q = 0; q < AX::kWin; ++q) win[q] = ld<TT>(wbase + r * TIWP + q);
+        for (int q = 0; q < AX::kWin; ++q) win[q] = to_acc<TT>(*(wbase + r * TIWP + q));
 #pragma unroll
         for (int i = 0; i < kPatch; ++i) {
 #pragma unroll
@@ -131,15 +125,15 @@ __device__ __forceinline__ void patch_compute_store_impl(const UpfirArgs& p, con
         } else {
 #pragma unroll
             for (int j = 0; j < kPatch; ++j)
-                if (ox0 + j < p.out_w) st<T>(rowp + j, acc[i][j]);
+                if (ox0 + j < p.out_w) rowp[j] = from_acc<T>(acc[i][j]);
         }
     }
 }
 
 template <typename T, int UX, int UY, int DX, int DY, int FW, int FH, int PHX, int PHY, int PITCH>
-__device__ __forceinline__ void patch_compute_store(const UpfirArgs& p, const typename AccT<T>::type* __restrict__ tile,
-                                                    const typename AccT<T>::type (&fk)[FH][FW], int n, int c, int ox_t, int oy_t) {
-    patch_compute_store_impl<T, typename AccT<T>::type, UX, UY, DX, DY, FW, FH, PHX, PHY, PITCH>(p, tile, fk, n, c, ox_t, oy_t);
+__device__ __forceinline__ void patch_compute_store(const UpfirArgs& p, const typename Acc<T>::type* __restrict__ tile,
+                                                    const typename Acc<T>::type (&fk)[FH][FW], int n, int c, int ox_t, int oy_t) {
+    patch_compute_store_impl<T, typename Acc<T>::type, UX, UY, DX, DY, FW, FH, PHX, PHY, PITCH>(p, tile, fk, n, c, ox_t, oy_t);
 }
 template <int UX, int UY, int DX, int DY, int FW, int FH, int PHX, int PHY, int PITCH>
 __device__ __forceinline__ void patch_compute_store_h(const UpfirArgs& p, const __half* __restrict__ tile, const float (&fk)[FH][FW],
@@ -151,7 +145,7 @@ __device__ __forceinline__ void patch_compute_store_h(const UpfirArgs& p, const 
 // the tile origin; the 0..3 surplus columns are absorbed by the row pitch and the window base is shifted accordingly.
 template <typename T, int UX, int UY, int DX, int DY, int FW, int FH, int PHX, int PHY, bool kVec>
 __global__ void __launch_bounds__(256) upfirdn2d_patch_kernel(const UpfirArgs p, int tiles_x, int tiles_y) {
-    using S = typename AccT<T>::type;
+    using S = typename Acc<T>::type;
     using AX = Axis<UX, DX, FW, PHX>;
     using AY = Axis<UY, DY, FH, PHY>;
     constexpr int TIW = AX::kTileIn, TIH = AY::kTileIn;
@@ -202,7 +196,7 @@ __global__ void __launch_bounds__(256) upfirdn2d_patch_kernel(const UpfirArgs p,
                 const int ty = i / TIW, tx = i - ty * TIW;
                 const int gx = ix_t + tx, gy = iy_t + ty;
                 S v = 0;
-                if ((unsigned)gx < (unsigned)p.in_w && (unsigned)gy < (unsigned)p.in_h) v = ld<T>(xin + gy * p.ish + gx);
+                if ((unsigned)gx < (unsigned)p.in_w && (unsigned)gy < (unsigned)p.in_h) v = to_acc<T>(*(xin + gy * p.ish + gx));
                 tile[ty * TIWP + tx] = v;
             }
         }
@@ -236,7 +230,7 @@ __global__ void __launch_bounds__(256) upfirdn2d_patch_tma_kernel(const UpfirArg
     using GM = TmaGeom<T, UX, UY, DX, DY, FW, FH, PHX, PHY>;
     using AX = typename GM::AX;
     using AY = typename GM::AY;
-    static_assert(sizeof(T) == sizeof(typename AccT<T>::type) || sizeof(T) == 2, "fp32 / fp16 only");
+    static_assert(sizeof(T) == sizeof(typename Acc<T>::type) || sizeof(T) == 2, "fp32 / fp16 only");
     static_assert((kTile * DX / UX) % GM::kVec == 0, "tile origins must keep the 16-byte phase of the box origin");
     extern __shared__ unsigned char tma_raw[];
     unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(tma_raw) + 127) & ~(uintptr_t)127);
@@ -302,7 +296,7 @@ __global__ void __launch_bounds__(256) upfirdn2d_patch_tma_kernel(const UpfirArg
 // generic: any strides / filter / factors.  Thread order follows the fastest-varying output stride.
 template <typename T>
 __global__ void __launch_bounds__(256) upfirdn2d_generic_kernel(const UpfirArgs p, int c_fastest) {
-    using S = typename AccT<T>::type;
+    using S = typename Acc<T>::type;
     const long long total = (long long)p.out_w * p.out_h * p.in_c * p.in_n;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         int ox, oy, c, n;
@@ -323,10 +317,11 @@ __global__ void __launch_bounds__(256) upfirdn2d_generic_kernel(const UpfirArgs 
                 if (ix < 0 || bx + kx < 0) continue;
                 if (ix >= p.in_w) break;
                 const int sx = p.flip ? kx : p.fw - 1 - kx;
-                acc += (S)p.f[sy * p.fsh + sx * p.fsw] * ld<T>(xin + iy * p.ish + ix * p.isw);
+                acc += (S)p.f[sy * p.fsh + sx * p.fsw] * to_acc<T>(*(xin + iy * p.ish + ix * p.isw));
             }
         }
-        st<T>((T*)p.y + n * p.osn + c * p.osc + oy * p.osh + ox * p.osw, acc * (S)p.gain);
+        T* yout = (T*)p.y + n * p.osn + c * p.osc + oy * p.osh + ox * p.osw;
+        *yout = from_acc<T>(acc * (S)p.gain);
     }
 }
 
@@ -376,7 +371,7 @@ static int launch_patch(const UpfirArgs& p, cudaStream_t st_) {
             if (rc != IDE3D_UNSUPPORTED) return rc;
         }
     }
-    using S = typename AccT<T>::type;
+    using S = typename Acc<T>::type;
     using AX = Axis<UX, DX, FW, PHX>;
     using AY = Axis<UY, DY, FH, PHY>;
     bool vec = false;
@@ -416,23 +411,6 @@ static int dispatch_phase(const UpfirArgs& p, cudaStream_t s) {
 // (kWin x kWin pixels, e.g. 7x7 for the up=1 FIR, 3x3 for 2x upsampling) is read with one vector load per pixel straight
 // from L1/L2 -- consecutive threads take consecutive channel vectors of the same patch, so every load and store of a warp
 // is one contiguous run along C.  No shared memory, no divisions / bounds checks per tap.
-template <typename T> struct V4;
-template <> struct V4<float> {
-    static __device__ __forceinline__ void ld(const float* p, float (&o)[4]) { const float4 t = __ldg(reinterpret_cast<const float4*>(p)); o[0] = t.x; o[1] = t.y; o[2] = t.z; o[3] = t.w; }
-    static __device__ __forceinline__ void st(float* p, const float (&o)[4]) { __stcs(reinterpret_cast<float4*>(p), make_float4(o[0], o[1], o[2], o[3])); }
-};
-template <> struct V4<__half> {
-    static __device__ __forceinline__ void ld(const __half* p, float (&o)[4]) {
-        const uint2 t = __ldg(reinterpret_cast<const uint2*>(p));
-        const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&t.x)), b = __half22float2(*reinterpret_cast<const __half2*>(&t.y));
-        o[0] = a.x; o[1] = a.y; o[2] = b.x; o[3] = b.y;
-    }
-    static __device__ __forceinline__ void st(__half* p, const float (&o)[4]) {
-        const __half2 a = __floats2half2_rn(o[0], o[1]), b = __floats2half2_rn(o[2], o[3]);
-        __stcs(reinterpret_cast<uint2*>(p), make_uint2(*reinterpret_cast<const unsigned*>(&a), *reinterpret_cast<const unsigned*>(&b)));
-    }
-};
-
 // What follows the FIR in the channels_last kernels.  kPlain: nothing, or the skip add with every tensor of type T; kEpi: the
 // modconv tail with its operands of type T; kEpiF32: the tail with float32 operands (scale, noise, bias, scale2) on fp16 x / y / y2;
 // kAddF16: the skip add of an fp16 `add` to float32 x / y / bias.
@@ -461,14 +439,14 @@ __device__ __forceinline__ void cl_patch_body(const UpfirArgs& p, const float (&
         // loads in flight
         const TA* ain = (const TA*)p.add + n * p.asn + cv * 4;
         float bv[4] = {0.f, 0.f, 0.f, 0.f};
-        if (p.bias != nullptr) V4<T>::ld((const T*)p.bias + cv * 4, bv);
+        if (p.bias != nullptr) load_vec_ro((const T*)p.bias + cv * 4, 0, bv);
 #pragma unroll
         for (int a = 0; a < kPatch; ++a) {
 #pragma unroll
             for (int b = 0; b < kPatch; ++b)
                 if (oy0 + a < p.out_h && ox0 + b < p.out_w) {
                     float av[4];
-                    V4<TA>::ld(ain + (oy0 + a) * p.ash + (ox0 + b) * p.asw, av);
+                    load_vec_ro(ain + (oy0 + a) * p.ash + (ox0 + b) * p.asw, 0, av);
 #pragma unroll
                     for (int c = 0; c < 4; ++c) acc[a][b][c] = av[c] + bv[c];
                 }
@@ -500,9 +478,9 @@ __device__ __forceinline__ void cl_patch_body(const UpfirArgs& p, const float (&
     T* yout = (T*)p.y + n * p.osn + cv * 4;
     if constexpr (kMode == kEpi || kMode == kEpiF32) {
         float dv[4] = {1.f, 1.f, 1.f, 1.f}, bv[4] = {0.f, 0.f, 0.f, 0.f}, d2[4] = {1.f, 1.f, 1.f, 1.f};
-        if (p.scale != nullptr) V4<TP>::ld((const TP*)p.scale + (long long)n * p.in_c + cv * 4, dv);
-        if (p.bias != nullptr) V4<TP>::ld((const TP*)p.bias + cv * 4, bv);
-        if (p.y2 != nullptr) V4<TP>::ld((const TP*)p.scale2 + (long long)n * p.in_c + cv * 4, d2);
+        if (p.scale != nullptr) load_vec_ro((const TP*)p.scale + (long long)n * p.in_c + cv * 4, 0, dv);
+        if (p.bias != nullptr) load_vec_ro((const TP*)p.bias + cv * 4, 0, bv);
+        if (p.y2 != nullptr) load_vec_ro((const TP*)p.scale2 + (long long)n * p.in_c + cv * 4, 0, d2);
         const TP* nz = (p.noise != nullptr) ? (const TP*)p.noise + (p.noise_batch == 1 ? 0ll : (long long)n * p.out_h * p.out_w) : nullptr;
         T* y2out = (p.y2 != nullptr) ? (T*)p.y2 + n * p.osn + cv * 4 : nullptr;
 #pragma unroll
@@ -511,7 +489,7 @@ __device__ __forceinline__ void cl_patch_body(const UpfirArgs& p, const float (&
 #pragma unroll
             for (int b = 0; b < kPatch; ++b) {
                 if (ox0 + b >= p.out_w) continue;
-                const float nv = nz ? ld<TP>(nz + (long long)(oy0 + a) * p.out_w + (ox0 + b)) : 0.f;
+                const float nv = nz ? to_acc<TP>(*(nz + (long long)(oy0 + a) * p.out_w + (ox0 + b))) : 0.f;
                 float v[4];
 #pragma unroll
                 for (int c = 0; c < 4; ++c) {
@@ -523,11 +501,11 @@ __device__ __forceinline__ void cl_patch_body(const UpfirArgs& p, const float (&
                     v[c] = t;
                 }
                 const long long o = (long long)(oy0 + a) * p.osh + (long long)(ox0 + b) * p.osw;
-                if (p.y != nullptr) V4<T>::st(yout + o, v);
+                if (p.y != nullptr) store_vec_cs(yout + o, 0, v);
                 if (y2out != nullptr) {
 #pragma unroll
                     for (int c = 0; c < 4; ++c) v[c] *= d2[c];
-                    V4<T>::st(y2out + o, v);
+                    store_vec_cs(y2out + o, 0, v);
                 }
             }
         }
@@ -537,7 +515,7 @@ __device__ __forceinline__ void cl_patch_body(const UpfirArgs& p, const float (&
             if (oy0 + a >= p.out_h) break;
 #pragma unroll
             for (int b = 0; b < kPatch; ++b)
-                if (ox0 + b < p.out_w) V4<T>::st(yout + (oy0 + a) * p.osh + (ox0 + b) * p.osw, acc[a][b]);
+                if (ox0 + b < p.out_w) store_vec_cs(yout + (oy0 + a) * p.osh + (ox0 + b) * p.osw, 0, acc[a][b]);
         }
     }
 }
@@ -578,7 +556,7 @@ __global__ void __launch_bounds__(256) upfirdn2d_cl_patch_kernel(const UpfirArgs
         const T* xin = (const T*)p.x + (long long)n * p.isn + cv * 4;
         cl_patch_body<T, UX, UY, DX, DY, FW, FH, PHX, PHY, kMode>(p, fk, n, cv, ox0, oy0, [&](int r, int q, float (&w)[4]) {
             const int gy = iy0 + r, gx = ix0 + q;
-            if ((unsigned)gy < (unsigned)p.in_h && (unsigned)gx < (unsigned)p.in_w) V4<T>::ld(xin + gy * p.ish + gx * p.isw, w);
+            if ((unsigned)gy < (unsigned)p.in_h && (unsigned)gx < (unsigned)p.in_w) load_vec_ro(xin + gy * p.ish + gx * p.isw, 0, w);
             else { w[0] = 0.f; w[1] = 0.f; w[2] = 0.f; w[3] = 0.f; }
         });
     }
@@ -608,18 +586,6 @@ struct ClTmaGeom {
     static constexpr int kSmem = kStages * kTileBytes + 128 + 128;
     static_assert(kCV * PX * PY == 256, "one thread per (channel vector, patch)");
 };
-template <typename T> struct V4s;
-template <> struct V4s<float> {
-    static __device__ __forceinline__ void ld(const float* p, float (&o)[4]) { const float4 t = *reinterpret_cast<const float4*>(p); o[0] = t.x; o[1] = t.y; o[2] = t.z; o[3] = t.w; }
-};
-template <> struct V4s<__half> {
-    static __device__ __forceinline__ void ld(const __half* p, float (&o)[4]) {
-        const uint2 t = *reinterpret_cast<const uint2*>(p);
-        const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&t.x)), b = __half22float2(*reinterpret_cast<const __half2*>(&t.y));
-        o[0] = a.x; o[1] = a.y; o[2] = b.x; o[3] = b.y;
-    }
-};
-
 template <typename T, int UX, int UY, int DX, int DY, int FW, int FH, int PHX, int PHY, int kMode, int CB>
 __global__ void __launch_bounds__(256, 2) upfirdn2d_cl_tma_kernel(const UpfirArgs p, int tiles_x, int tiles_y, int cblocks,
                                                                const __grid_constant__ CUtensorMap tmap) {
@@ -671,7 +637,7 @@ __global__ void __launch_bounds__(256, 2) upfirdn2d_cl_tma_kernel(const UpfirArg
         const int ox0 = ox_t + ptx * kPatch, oy0 = oy_t + pty * kPatch;
         if (ox0 < p.out_w && oy0 < p.out_h)
             cl_patch_body<T, UX, UY, DX, DY, FW, FH, PHX, PHY, kMode>(p, fk, n, cb * (kClCB / 4) + cvl, ox0, oy0, [&](int r, int q, float (&w)[4]) {
-                V4s<T>::ld(tile + (r * GM::BW + q) * kClCB, w);
+                load_vec(tile + (r * GM::BW + q) * kClCB, 0, w);
             });
         __syncthreads();                                                     // every thread is done with stage `cur`
         const long long nxt = t + (long long)NST * gridDim.x;
@@ -730,16 +696,13 @@ static int launch_cl_patch(const UpfirArgs& p, cudaStream_t st_) {
     }
     const int patches_x = ceil_div(p.out_w, kPatch), patches_y = ceil_div(p.out_h, kPatch);
     const long long total = (long long)patches_x * patches_y * p.in_n * (p.in_c >> 2);
-    long long grid = ceil_div<long long>(total, 256);
-    const long long cap = (long long)sm_count() * 8;
-    if (grid > cap) grid = cap;
     void (*kern)(const UpfirArgs, int, int) = p.epi ? upfirdn2d_cl_patch_kernel<T, UX, UY, DX, DY, FW, FH, PHX, PHY, kEpi>
                                                     : upfirdn2d_cl_patch_kernel<T, UX, UY, DX, DY, FW, FH, PHX, PHY, kPlain>;
     if constexpr (std::is_same<T, __half>::value)
         if (p.mixed) kern = upfirdn2d_cl_patch_kernel<T, UX, UY, DX, DY, FW, FH, PHX, PHY, kEpiF32>;
     if constexpr (std::is_same<T, float>::value)
         if (p.mixed) kern = upfirdn2d_cl_patch_kernel<T, UX, UY, DX, DY, FW, FH, PHX, PHY, kAddF16>;
-    kern<<<(unsigned)grid, 256, 0, st_>>>(p, patches_x, patches_y);
+    kern<<<capped_grid(ceil_div<long long>(total, 256), 8), 256, 0, st_>>>(p, patches_x, patches_y);
     IDE3D_CHECK_LAUNCH("upfirdn2d_cl_patch_kernel");
     return IDE3D_OK;
 }
@@ -763,7 +726,7 @@ static int dispatch_phase_cl(const UpfirArgs& p, cudaStream_t s) {
 // (adjacent outputs share them).  Any filter / factors; coalesced along C.
 template <typename T>
 __global__ void __launch_bounds__(256) upfirdn2d_cl_kernel(const UpfirArgs p) {
-    using S = typename AccT<T>::type;
+    using S = typename Acc<T>::type;
     const int c4n = p.in_c >> 2;
     const long long total = (long long)p.out_w * p.out_h * p.in_n * c4n;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -787,22 +750,19 @@ __global__ void __launch_bounds__(256) upfirdn2d_cl_kernel(const UpfirArgs p) {
                 if (ix >= p.in_w) break;
                 const S w = (S)p.f[sy * p.fsh + (p.flip ? kx : p.fw - 1 - kx) * p.fsw];
                 const T* px = xin + iy * p.ish + ix * p.isw;
-                a0 += w * ld<T>(px); a1 += w * ld<T>(px + 1); a2 += w * ld<T>(px + 2); a3 += w * ld<T>(px + 3);
+                a0 += w * to_acc<T>(px[0]); a1 += w * to_acc<T>(px[1]); a2 += w * to_acc<T>(px[2]); a3 += w * to_acc<T>(px[3]);
             }
         }
         T* py = (T*)p.y + n * p.osn + oy * p.osh + ox * p.osw + c4 * 4;
         const S g = (S)p.gain;
-        st<T>(py, a0 * g); st<T>(py + 1, a1 * g); st<T>(py + 2, a2 * g); st<T>(py + 3, a3 * g);
+        py[0] = from_acc<T>(a0 * g); py[1] = from_acc<T>(a1 * g); py[2] = from_acc<T>(a2 * g); py[3] = from_acc<T>(a3 * g);
     }
 }
 
 template <typename T>
 static int launch_cl(const UpfirArgs& p, cudaStream_t s) {
     const long long total = (long long)p.out_w * p.out_h * p.in_n * (p.in_c >> 2);
-    long long grid = ceil_div<long long>(total, 256);
-    const long long cap = (long long)sm_count() * 16;
-    if (grid > cap) grid = cap;
-    upfirdn2d_cl_kernel<T><<<(unsigned)grid, 256, 0, s>>>(p);
+    upfirdn2d_cl_kernel<T><<<capped_grid(ceil_div<long long>(total, 256), 16), 256, 0, s>>>(p);
     IDE3D_CHECK_LAUNCH("upfirdn2d_cl_kernel");
     return IDE3D_OK;
 }
@@ -810,11 +770,8 @@ static int launch_cl(const UpfirArgs& p, cudaStream_t s) {
 template <typename T>
 static int launch_generic(const UpfirArgs& p, cudaStream_t s) {
     const long long total = (long long)p.out_w * p.out_h * p.in_c * p.in_n;
-    long long grid = ceil_div<long long>(total, 256);
-    const long long cap = (long long)sm_count() * 16;
-    if (grid > cap) grid = cap;
     const int c_fastest = (p.osc == 1 && p.osw != 1) ? 1 : 0;
-    upfirdn2d_generic_kernel<T><<<(unsigned)grid, 256, 0, s>>>(p, c_fastest);
+    upfirdn2d_generic_kernel<T><<<capped_grid(ceil_div<long long>(total, 256), 16), 256, 0, s>>>(p, c_fastest);
     IDE3D_CHECK_LAUNCH("upfirdn2d_generic_kernel");
     return IDE3D_OK;
 }

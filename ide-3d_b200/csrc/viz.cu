@@ -376,8 +376,7 @@ extern "C" int ide3d_viz_image(const void* x, int dtype, int c, int h, int w, in
     ImageArgs a{c, h, w, base_channel, sel_channels, depth != 0, normalize != 0, out_channels, chunks, stride_c, stride_h, stride_w, gain,
                 out, out_stride_h, out_stride_w, out_stride_c, stats, part};
     const long long npix = (long long)h * w;
-    const unsigned igrid = (unsigned)(ceil_div<long long>(npix, kImgThreads) < 8LL * sm_count() ? ceil_div<long long>(npix, kImgThreads)
-                                                                                                 : 8LL * sm_count());
+    const unsigned igrid = capped_grid(ceil_div<long long>(npix, kImgThreads), 8);
     if (dtype == IDE3D_F32) {
         viz_reduce_kernel<float><<<rgrid, kRedThreads, 0, st>>>(static_cast<const float*>(x), h, w, stride_c, stride_h, stride_w, chunks, part);
         IDE3D_CHECK_LAUNCH("viz_reduce_kernel");
@@ -460,9 +459,7 @@ extern "C" int ide3d_viz_fft(const void* x, int dtype, int c, int h, int w, int6
     viz_fft_sum_kernel<<<a.parts, kFftThreads, 0, st>>>(a);
     IDE3D_CHECK_LAUNCH("viz_fft_sum_kernel");
     const long long npix = (long long)N * N;
-    const unsigned pgrid = (unsigned)(ceil_div<long long>(npix, kFftThreads) < 4LL * sm_count() ? ceil_div<long long>(npix, kFftThreads)
-                                                                                                : 4LL * sm_count());
-    viz_fft_panel_kernel<<<pgrid, kFftThreads, 0, st>>>(a);
+    viz_fft_panel_kernel<<<capped_grid(ceil_div<long long>(npix, kFftThreads), 4), kFftThreads, 0, st>>>(a);
     IDE3D_CHECK_LAUNCH("viz_fft_panel_kernel");
     return IDE3D_OK;
 }
